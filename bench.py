@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- tiles/sec of the HoVer-Net tile hot path (infer_step + post_proc.process per patch).
 
-    python bench.py --gpus N --steps K --warmup W                 # this repo (libhvn, sm_100a kernels)
+    python bench.py --gpus N --steps K --warmup W                 # this repo (libhvn, sm_90a kernels)
     python bench.py --impl reference --gpus N --steps K ...       # the reference path on the same box
     python bench.py --workload fast64|tile4k|wsi40k ...           # the other BASELINE.json configs
 
@@ -15,11 +15,17 @@ every rank its own batch (weak scaling) and rank 0 receives the packed instance 
 
 `value`   : device-timed (CUDA events on the library's stream), inputs resident in HBM, gather included at N > 1.
 `e2e`     : same metric through the host-buffer C-ABI call (`hvn_forward_postproc`): pinned host uint8 in,
-            inst_map + instance table out, copies (and at N > 1 the gather) inside the timed region.
-`roofline`: dominant kernel class = the tcgen05 convolution; algorithmic 2*MACs of the reference graph per launch /
-            its measured launch time (per-launch CUDA events, kernels serialised) vs MEASURED_PEAKS.json.
+            inst_map + instance table out (the float maps are not requested here, unlike the resident path), copies
+            (and at N > 1 the gather) inside the timed region.
+`roofline`: dominant kernel class = the wgmma convolution; algorithmic 2*MACs of the reference graph per launch /
+            its measured launch time (per-launch CUDA events, kernels serialised) vs MEASURED_PEAKS.json, else the
+            H100 SXM data sheet (dense BF16, HBM3) -- a bound, not a rate this code has reached.
+`--dump-outputs DIR`: after the timed steps, what the timed path returned in its last step (the CNN's float maps,
+            inst maps, instance tables, row counts; tile4k: the stitched map, inst map and instance table; wsi40k: the
+            instance table of the JSON) as DIR/<name>.npy in float32 / float64, at most 64 MB in all (larger outputs:
+            a fixed, seeded sample of patches / image rows, indices in DIR/sample_index.npy).
 `roofline_postproc`: the post-processing half of the metric: algorithmic bytes (C*4 B read + 4 B written per pixel)
-            / device time vs the measured HBM copy bandwidth, on the CNN's own output maps and on nuclei-like maps.
+            / device time vs the HBM bandwidth, on the CNN's own output maps and on nuclei-like maps.
 `--impl reference` (default arm = what north_star names): the unmodified reference graph restated in torch
             (oracle/hovernet_torch.py, pinned bit-for-bit against the reference) on PyTorch-CUDA with stock settings,
             overlapped with the reference-faithful CPU post-processing in a pool of os.cpu_count() processes
@@ -97,27 +103,39 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
-def measured_traffic(kernel_class, mode):
-    """dram__bytes_read+write per launch of the dominant kernel from the committed ncu capture of this workload's
-    mode (profiles/*_traffic*.json, newest first); null when no capture of that mode is committed."""
-    try:
-        import glob
-        for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "*traffic*.json")), reverse=True):
-            t = json.load(open(path))
-            if t.get("mode", "fast") != mode:
-                continue
-            # the tcgen05 convolution class = k_conv_tc + its A-resident (k_conv_ar) and row-stacked (k_conv_rs) variants
-            names = ("k_conv_tc", "k_conv_ar", "k_conv_rs") if kernel_class == "conv_tc" else ("k_conv_ref",)
-            ks = [t["kernels"][n] for n in names if n in t["kernels"]]
-            k = {"dram_bytes": sum(x["dram_bytes"] for x in ks), "launches": sum(x["launches"] for x in ks)}
-            return {"dram_bytes_per_launch": k["dram_bytes"] / k["launches"], "launches": k["launches"],
-                    "batch": t["batch"], "source": "profiles/" + os.path.basename(path) + " (" + t["command"] + ")"}
-    except Exception:
-        pass
-    return None
+DUMP_LIMIT = 64 << 20
+
+
+def inst_rows(info):
+    """Instance dict (tile / WSI output format) -> float64 [n, 9] rows: id, bbox (rmin, cmin, rmax, cmax), centroid (x, y),
+    type, type_prob (-1 when untyped), in id order."""
+    rows = [[float(k)] + [float(x) for x in np.ravel(v["bbox"])] + [float(x) for x in np.ravel(v["centroid"])] +
+            [-1.0 if v.get(t) is None else float(v[t]) for t in ("type", "type_prob")]
+            for k, v in sorted(info.items(), key=lambda kv: int(kv[0]))]
+    return np.asarray(rows, np.float64).reshape(-1, 9)
+
+
+def dump_outputs(out_dir, arrays, tables=None):
+    """Writes {name: array} as out_dir/<name>.npy (integers as float64, floats as float32), `tables` whole.  The arrays
+    share their first axis (patches, or image rows); when they would exceed DUMP_LIMIT bytes, a fixed seeded sample of
+    that axis is written instead, its indices in sample_index.npy."""
+    tables = {k: np.asarray(v, np.float64) for k, v in (tables or {}).items()}
+    conv = {k: (v.astype(np.float32) if np.issubdtype(v.dtype, np.floating) else v.astype(np.float64)) for k, v in arrays.items()}
+    n = next(iter(conv.values())).shape[0]
+    per_row = sum(v[:1].nbytes for v in conv.values())
+    keep = min(n, max(1, (DUMP_LIMIT - 8 * n - sum(t.nbytes for t in tables.values())) // max(1, per_row)))
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in tables.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    if keep < n:
+        idx = np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+        conv = {k: v[idx] for k, v in conv.items()}
+        np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+    for k, v in conv.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.ascontiguousarray(v))
 
 
 def dist_env():
@@ -154,7 +172,7 @@ def workload_config(args, world, note=None):
            "name": args.workload, "mode": args.mode, "nr_types": args.nr_types, "batch_per_gpu": args.batch,
            "patch": args.patch,
            "parallelism": "tiles sharded per rank (dp%d), end-of-batch NCCL gather of the packed instance tables" % world,
-           "l2": "per-step activations (%.0f GB at %.2f GB/patch) exceed the 126 MB L2; a 256 MB buffer is also written "
+           "l2": "per-step activations (%.0f GB at %.2f GB/patch) exceed the 50 MB L2; a 256 MB buffer is also written "
                  "between timed steps" % (0.5 * args.batch, 0.5)}
     if note:
         cfg["note"] = note
@@ -359,6 +377,7 @@ def run_ours(args):
 
     # device-resident buffers are torch tensors (so NCCL can gather them); libhvn gets raw pointers
     d_img = torch.from_numpy(x).to(dev)
+    d_pred = torch.empty((B, oh, ow, oc), dtype=torch.float32, device=dev)   # the NP/HV(/TP) maps infer_step returns
     d_inst = torch.empty((B, oh, ow), dtype=torch.int32, device=dev)
     d_tab = torch.zeros((B, max_rows, 10), dtype=torch.int64, device=dev)
     d_nr = torch.zeros((B,), dtype=torch.int32, device=dev)
@@ -367,8 +386,8 @@ def run_ours(args):
     torch.cuda.synchronize()
 
     def step_resident():
-        ctx.forward_postproc_dev(d_img.data_ptr(), B, S, S, None, d_inst.data_ptr(), d_tab.data_ptr(), max_rows,
-                                 d_nr.data_ptr())
+        ctx.forward_postproc_dev(d_img.data_ptr(), B, S, S, d_pred.data_ptr(), d_inst.data_ptr(), d_tab.data_ptr(),
+                                 max_rows, d_nr.data_ptr())
         return pg.launch(d_tab, d_nr)     # pack on the library stream + async all_gather (overlaps the next step)
 
     def barrier():
@@ -399,6 +418,9 @@ def run_ours(args):
         step_ms.append(ctx.timer_stop())
     barrier()
     wall = time.perf_counter() - t_wall
+    if args.dump_outputs and rank == 0:   # the last timed step's results, before the passes below reuse the buffers
+        dump_outputs(args.dump_outputs, {"pred_map": d_pred.cpu().numpy(), "inst_map": d_inst.cpu().numpy(),
+                                         "inst_table": d_tab.cpu().numpy(), "n_rows": d_nr.cpu().numpy()})
     launches = ctx.counter("kernel_launches") - launches0
     total_ms = float(np.sum(step_ms))
     got = pg.rows(k)
@@ -482,7 +504,7 @@ def run_ours(args):
         dom = "conv_tc" if prof["conv_tc"]["launches"] > 0 else "conv_ref"
         d = prof[dom]
         ach = (d["gflop"] / 1e3) / (d["ms"] / 1e3) if d["ms"] > 0 else 0.0  # TFLOP/s
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+        peak = pk["bf16_tflops"]
         value = world * B * args.steps / (total_ms / 1e3)
         e2e_v = world * B * args.steps / (e2e_total / 1e3)
         pp_bytes = B * oh * ow * (oc * 4 + 4)
@@ -500,12 +522,11 @@ def run_ours(args):
             "gpu_launches": int(launches),
             "clocks": sampler.summary(),
             "roofline": {"bound": "tensor", "kernel": dom, "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-                         "frac": ach / peak if peak else None, "peak_source": pk_kind + " bf16_tflops_sustained",
+                         "frac": ach / peak if peak else None, "peak_source": pk_kind + " bf16_tflops",
                          "algorithmic_gflop_per_launch": d["gflop"] / max(1, d["launches"]),
                          "avg_launch_ms": d["ms"] / max(1, d["launches"]), "launches_per_step": d["launches"],
-                         "traffic": measured_traffic(dom, mode),
                          "note": "algorithmic 2*MACs of the reference graph; every product is formed three times in "
-                                 "fp16 (hi*hi+hi*lo+lo*hi, issued as two or three MMA instructions per K-step), so frac <= 1/3 "
+                                 "fp16 (hi*hi+hi*lo+lo*hi, three wgmma instructions per K-step), so frac <= 1/3 "
                                  "by construction"},
             "roofline_postproc": {"bound": "hbm", "unit": "GB/s", "peak": hbm, "peak_source": pk_kind + " hbm_gbs",
                                   "algorithmic_bytes_per_step": pp_bytes,
@@ -588,6 +609,9 @@ def run_tile(args):
     if rank == 0:
         pred, inst, info = res
         npatch = rows * cols
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"inst_map": inst, **({"pred_map": pred} if pred is not None else {})},
+                         {"inst_table": inst_rows(info)})
         import hashlib
         line = {"metric": "tiles/sec", "value": npatch * args.steps / total, "unit": "tiles/s", "n_gpus": world,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": total / args.steps * 1e3,
@@ -643,12 +667,26 @@ def run_wsi(args):
                 "save_thumb": False, "save_mask": False}
     if world > 1:
         dist.barrier()
+
+    def one_pass():   # a fresh output and cache each pass: the driver skips slides whose JSON already exists
+        if world > 1:
+            dist.barrier()
+        if rank == 0:
+            shutil.rmtree(work + "/out", ignore_errors=True)
+            os.makedirs(work + "/out")
+        shutil.rmtree(run_args["cache_path"], ignore_errors=True)
+        if world > 1:
+            dist.barrier()
+        t0 = time.perf_counter()
+        mgr.process_wsi_list(run_args)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t0
+
+    for _ in range(args.warmup):
+        one_pass()
     sampler = ClockSampler(local)
     sampler.start()
-    t0 = time.perf_counter()
-    mgr.process_wsi_list(run_args)
-    torch.cuda.synchronize()
-    t = torch.tensor([time.perf_counter() - t0], dtype=torch.float64, device="cuda")
+    t = torch.tensor([sum(one_pass() for _ in range(args.steps))], dtype=torch.float64, device="cuda")
     sampler.stop_flag.set()
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -656,18 +694,21 @@ def run_wsi(args):
     if rank == 0:
         js = open(work + "/out/slide.json", "rb").read()
         n_step = (args.size - (win - out)) // out + 1
-        line = {"metric": "tiles/sec", "value": n_step * n_step / total, "unit": "tiles/s", "n_gpus": world, "steps": 1,
-                "warmup": 0, "ms_per_step": total * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
+        line = {"metric": "tiles/sec", "value": n_step * n_step * args.steps / total, "unit": "tiles/s", "n_gpus": world,
+                "steps": args.steps, "warmup": args.warmup, "ms_per_step": total / args.steps * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
                 "dtype": "f16x3-split; post-proc int32/f64", "data": "synthetic",
                 "config": {"workload": "BASELINE configs[4]: %dx%d synthetic slide through the WSI driver, %s mode, %d patches, "
                                        "chunks of 10000, 2048 tiles + boundary + cross phases, %d rank(s), JSON on rank 0" % (
                                            args.size, args.size, mode, n_step * n_step, world),
                            "name": "wsi40k", "mode": mode, "nr_types": nt, "patches": n_step * n_step},
-                "e2e": {"value": n_step * n_step / total, "unit": "tiles/s", "h2d_bytes_per_step": int(args.size) ** 2 * 3,
+                "e2e": {"value": n_step * n_step * args.steps / total, "unit": "tiles/s", "h2d_bytes_per_step": int(args.size) ** 2 * 3,
                         "d2h_bytes_per_step": len(js), "note": "slide file in, JSON out (wall clock, max over ranks)"},
                 "gpu_launches": int(mgr.net.ctx.counter("kernel_launches")), "clocks": sampler.summary(),
                 "instances": len(json.loads(js)["nuc"]), "json_sha1": hashlib.sha1(js).hexdigest()}
         print(json.dumps(line))
+        if args.dump_outputs:   # the last timed pass's JSON as an instance table
+            dump_outputs(args.dump_outputs, {"n_instances": np.array([len(json.loads(js)["nuc"])])},
+                         {"inst_table": inst_rows(json.loads(js)["nuc"])})
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
@@ -697,7 +738,11 @@ def main():
     ap.add_argument("--cpu-threads", type=int, default=32)
     ap.add_argument("--ref-forward", default="cuda", choices=["cpu", "cuda"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32/float64, <= 64 MB in all)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs covers this repo's workloads")
     w = WORKLOADS[args.workload]
     args.stock = args.mode is None and args.nr_types is None and args.batch is None and args.size is None
     args.config = w["config"]

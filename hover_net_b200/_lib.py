@@ -1,5 +1,5 @@
 """ctypes binding of libhvn.so (include/hvn.h).  There is no CPU fallback: if the CUDA library is
-missing or no sm_100 device is present, every entry point raises."""
+missing or no sm_90 device is present, every entry point raises."""
 import ctypes
 import os
 

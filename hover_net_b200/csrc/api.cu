@@ -67,8 +67,8 @@ static int create_common(int device, hvn_ctx **out, const char *mode, int nr_typ
     HVN_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     HVN_CUDA(cudaGetDeviceProperties(&prop, device));
-    HVN_CHECK(prop.major == 10, HVN_ERR_CUDA,
-              std::string("libhvn is built for sm_100a only; device is ") + prop.name);
+    HVN_CHECK(prop.major == 9 && prop.minor == 0, HVN_ERR_CUDA,
+              std::string("libhvn is built for sm_90a only; device is ") + prop.name);
     if (with_model) c->model.reset(new Model(mode ? mode : "", nr_types));
     HVN_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     for (auto &e : c->ev) HVN_CUDA(cudaEventCreate(&e));
@@ -139,17 +139,8 @@ int hvn_set_option(hvn_ctx *c, const char *key, int64_t value) {
     else if (k == "branch_streams") { HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model"); c->model->branch_streams = (int)value; }
     else if (k == "tc_seg_chunks") tc_set_seg_chunks((int)value);
     else if (k == "tc_block_n") tc_set_block_n((int)value);
-    else if (k == "tc_res_tma") tc_set_res_tma((int)value);
     else if (k == "tc_xf_trunc") tc_set_xf_trunc((int)value);
-    else if (k == "tc_ar") tc_set_ar((int)value);
-    else if (k == "tc_lean_epi") tc_set_lean_epi((int)value);
-    else if (k == "tc_rowstack") tc_set_rowstack((int)value);
-    else if (k == "tc_xf_early") tc_set_xf_early((int)value);
     else if (k == "tc_prefetch") tc_set_prefetch((int)value);
-    else if (k == "tc_ar_min_chunks") tc_set_ar_min_chunks((int)value);
-    else if (k == "tc_ar_nres") tc_set_ar_nres((int)value);
-    else if (k == "tc_ar_min_wst") tc_set_ar_min_wst((int)value);
-    else if (k == "tc_res_tma_max_chunks") tc_set_res_tma_max_chunks((int)value);
     else if (k == "act_shift") {
         HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
         HVN_CHECK(value >= 0 && value <= 48, HVN_ERR_INVALID, "act_shift out of range (0..48)");
@@ -159,7 +150,6 @@ int hvn_set_option(hvn_ctx *c, const char *key, int64_t value) {
             if (c->model->finalized) c->model->finalize();  // re-derives the BN shifts / head weights; plans are rebuilt
         }
     }
-    else if (k == "tc_halo") { HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model"); c->model->tc_halo = (int)value; }
     else if (k == "profile") { c->profile = (int)value; if (c->model) c->model->profile_ops = value >= 3 ? 2 : (value >= 2 ? 1 : 0); }
     else throw Error(HVN_ERR_INVALID, "unknown option " + k);
     API_END

@@ -347,7 +347,7 @@ void Model::out_shape(int H, int W, int &oh, int &ow, int &oc) const {
 }
 
 // ------------------------------------------------------------------------------------------------
-// conv_path = 2: per-layer self test of the tcgen05 kernel against the CUDA-core referee
+// conv_path = 2: per-layer self test of the wgmma kernel against the CUDA-core referee
 __global__ void k_cmp_raw(const float *a, const float *b, int B, int h, int w, int c, long long sN, int sH, int sW,
                           unsigned int *out) {
     long long total = (long long)B * h * w * c;
@@ -422,9 +422,9 @@ void Model::selftest_conv(const Op &op, cudaStream_t s) {
     float f[4];
     memcpy(f, h_out, 16);
     char line[512];
-    snprintf(line, sizeof(line), "%-44s k%dx%d s%d cin%-4d cout%-4d %dx%d flat=%d box=%dx%d%s bn=%d | raw diff %.3e (ref %.3e) | split diff %.3e (ref %.3e)%s\n",
+    snprintf(line, sizeof(line), "%-44s k%dx%d s%d cin%-4d cout%-4d %dx%d flat=%d box=%dx%d bn=%d | raw diff %.3e (ref %.3e) | split diff %.3e (ref %.3e)%s\n",
              op.name.c_str(), op.cp.w.kh, op.cp.w.kw, op.cp.stride, op.cp.w.cin, op.cp.w.cout, op.cp.ho, op.cp.wo,
-             op.tc.flat, op.tc.bw, op.tc.bh, op.tc.halo ? "H" : "", op.tc.block_n, f[0], f[1], f[2], f[3],
+             op.tc.flat, op.tc.bw, op.tc.bh, op.tc.block_n, f[0], f[1], f[2], f[3],
              e == cudaSuccess ? "" : (std::string("  CUDA ERROR: ") + cudaGetErrorString(e)).c_str());
     debug_log += line;
     if (trace) { fputs(line, stderr); fflush(stderr); }
@@ -452,7 +452,7 @@ Plan &Model::plan(int B, int H, int W) {
     HVN_CHECK(finalized, -5, "weights not finalised (call hvn_finalize_weights)");
     HVN_CHECK(H == W, -1, "only square patches are supported (reference patch geometry is square)");
     std::string key = std::to_string(B) + "x" + std::to_string(H) + "x" + std::to_string(W) + "p" + std::to_string(conv_path) +
-                      "b" + std::to_string(branch_streams) + "x" + std::to_string(xform) + "f" + std::to_string(fuse_shortcut) + "u" + std::to_string(fuse_up2) + "h" + std::to_string(tc_halo);
+                      "b" + std::to_string(branch_streams) + "x" + std::to_string(xform) + "f" + std::to_string(fuse_shortcut) + "u" + std::to_string(fuse_up2);
     auto it = plans_.find(key);
     if (it != plans_.end()) return *it->second;
     std::unique_ptr<Plan> pl(new Plan());
@@ -665,7 +665,6 @@ Plan &Model::plan(int B, int H, int W) {
     cur_stream = 0;
     P.ops.push_back(head);
 
-    tc_set_halo(tc_halo);
     for (auto &op : P.ops) {
         P.flops += op.flops;
         if (op.kind == Op::CONV && conv_path != 1) tc_plan(op.cp, op.tc);
@@ -679,7 +678,7 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
     HVN_CHECK(B >= 1, -1, "empty batch");
     int oh, ow, oc;
     out_shape(H, W, oh, ow, oc);
-    if (chunk <= 0) chunk = 32;  // sub-batch size: large enough to fill 148 persistent CTAs on the thin decoder layers
+    if (chunk <= 0) chunk = 32;  // sub-batch size: large enough to fill 132 persistent CTAs on the thin decoder layers
     if (!side_[0]) {
         for (auto &st : side_) HVN_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
         HVN_CUDA(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
@@ -777,9 +776,9 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
                 char line[384];
                 const Op &o = *r.op;
                 if (o.kind == Op::CONV)
-                    snprintf(line, sizeof(line), "%-44s %-8s k%dx%d s%d cin%-4d cout%-4d out%dx%d box=%dx%d%s bn=%d %8.4f ms %8.2f GFLOP %7.1f TFLOP/s\n",
+                    snprintf(line, sizeof(line), "%-44s %-8s k%dx%d s%d cin%-4d cout%-4d out%dx%d box=%dx%d bn=%d %8.4f ms %8.2f GFLOP %7.1f TFLOP/s\n",
                              o.name.c_str(), r.cls, o.cp.w.kh, o.cp.w.kw, o.cp.stride, o.cp.w.cin, o.cp.w.cout, o.cp.ho, o.cp.wo,
-                             o.tc.bw, o.tc.bh, o.tc.halo ? "H" : "", o.tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f));
+                             o.tc.bw, o.tc.bh, o.tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f));
                 else
                     snprintf(line, sizeof(line), "%-44s %-8s %8.4f ms\n", o.name.c_str(), r.cls, ms);
                 debug_log += line;

@@ -63,13 +63,12 @@ class Model {
     std::map<std::string, int> index;
     std::map<std::string, std::vector<float>> host;
     bool finalized = false;
-    int tc_halo = 1;         // k x k stride-1 layers from one halo tile per channel block: 0 off, 1 where its 8 x 16 tiling fits, 2 all eligible
     int fuse_up2 = 0;        // 1: 2x upsample + skip add inside the conv epilogue; 0: separate streaming pass (faster)
     int fuse_shortcut = 1;   // fold each residual group's 1x1 shortcut into unit 0's conv3 (one GEMM over [a2 | x])
     int stem_tc = 1;         // stem (conv0) on the tensor core (k_conv0_tc); 0: CUDA-core k_conv0
     int xform = 1;           // fuse pre-activation BN+ReLU into the consuming 1x1 conv's A-operand load
     int branch_streams = 1;  // run the decoder branches on separate streams
-    int conv_path = 0;  // 0 auto (tcgen05 where eligible), 1 referee only, 2 auto + per-layer self test
+    int conv_path = 0;  // 0 auto (wgmma where eligible), 1 referee only, 2 auto + per-layer self test
     // Activations travel as fp16 hi + lo, finite up to 65504.  act_shift = s stores every activation as x * 2^-s:
     // the stem's BN scale, every BN shift and (inversely) the head weights absorb the factor, so the network function
     // is unchanged (powers of two are exact) while the representable range grows to 65504 * 2^s.  0 by default; raise
@@ -93,7 +92,7 @@ class Model {
     std::map<std::string, double> class_ms, class_flops;
     std::map<std::string, long long> class_launches;
     double last_flops = 0;  // algorithmic 2*MACs of the last forward()
-    std::string debug_log;  // conv_path == 2: per-layer tcgen05-vs-referee report of the last forward()
+    std::string debug_log;  // conv_path == 2: per-layer wgmma-vs-referee report of the last forward()
     void selftest_conv(const Op &op, cudaStream_t s);
 
   private:

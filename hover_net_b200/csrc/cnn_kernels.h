@@ -32,7 +32,7 @@ void launch_bnrelu(const RawRef &in, int B, const float *scale, const float *shi
 void launch_head(const HeadParams &P, cudaStream_t s);
 void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRef &out, cudaStream_t s);
 
-// tcgen05 path (conv_tc.cu).  tc_plan() decides eligibility and builds the TMA descriptors once per
+// wgmma path (conv_tc.cu).  tc_plan() decides eligibility and builds the TMA descriptors once per
 // (layer, buffer geometry); tc_launch() issues the kernel.
 struct TcPlan {
     bool ok = false;
@@ -42,28 +42,12 @@ struct TcPlan {
     int tiles_x = 0, tiles_y = 0;
     int block_n = 0;
     int flat = 0;                // 1x1 stride-1 dense view: M flattened over B*H*W
-    int res_tma = 0;             // residual tile fetched by TMA (tmap_a2_hi holds its fp32 map)
-    int rs = 0, rs_bw = 0, rs_bh = 0;   // row-stacked variant (k_conv_rs): A maps in tmap_a2_hi / lo, stacked weight maps below
-    unsigned char tmap_rs_w_hi[128], tmap_rs_w_lo[128];
-    int ar = 0, ar_gn = 1;       // A-resident variant (k_conv_ar): tmap_a2_lo = swizzled [32 px][32 ch] residual boxes; N-tiles per work unit
-    int halo = 0;                // k x k stride-1 layer served from one halo tile per 64-channel block
-    int halo_w = 0, halo_h = 0;  // halo extent in pixels (bw + kw - 1, bh + kh - 1)
 };
 bool tc_plan(const ConvParams &P, TcPlan &plan);
 void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s);
 void tc_set_block_n(int n);      // tuning knobs (0 = automatic)
 void tc_set_seg_chunks(int n);
-void tc_set_res_tma(int on);
-void tc_set_res_tma_max_chunks(int n);  // largest K (in 64-channel slices) served by the RT variant
-void tc_set_ar(int on);          // 1x1 + residual, K <= 256: A-resident kernel (1, default) or the RT variant (0)
-void tc_set_ar_min_chunks(int n);  // smallest K (in 64-channel slices) served by the A-resident kernel
-void tc_set_ar_nres(int n);      // residual regions per epilogue warp: upper limit (1..4)
-void tc_set_ar_min_wst(int n);   // ... while the weight ring keeps at least this many stages
 void tc_set_prefetch(int n);     // L2 prefetch distance in K-slices for flat (2-D map) operands, 0 = off
-void tc_set_rowstack(int on);    // grouped k x k layers on k_conv_rs (1, default) or the per-tap / HALO path (0)
-void tc_set_lean_epi(int on);    // k_conv_tc write-out with per-tile precomputed output offsets (1, default)
-void tc_set_xf_early(int on);    // XF: early raw-slot release + raw loads one slice ahead (1, default)
 void tc_set_xf_trunc(int on);    // XF transform warps: truncating hi/lo split (1, default) or round-to-nearest (0)
-void tc_set_halo(int mode);      // 0 off, 1 auto (where the 8 x 16 tiling fits the map), 2 every eligible layer
 
 }  // namespace hvn

@@ -1,4 +1,4 @@
-// Shared helpers for libhvn (sm_100a only).
+// Shared helpers for libhvn (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

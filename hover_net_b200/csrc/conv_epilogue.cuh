@@ -1,4 +1,4 @@
-// Fused convolution epilogue shared by the referee and the tcgen05 kernels:
+// Fused convolution epilogue shared by the referee and the wgmma kernels:
 // residual add, raw fp32 store, BN(scale/shift)+ReLU -> split fp16 store, or 2x nearest-neighbour
 // upsample + skip add -> split store (reference net_utils.py:263-265, net_desc.py:133-139).
 #pragma once
@@ -108,7 +108,7 @@ __device__ __forceinline__ void conv_epilogue4(const ConvParams &P, int n, int o
 }
 
 
-// ---- two-phase form used by the tcgen05 kernel: issue the (independent) global loads of several
+// ---- two-phase form: issue the (independent) global loads of several
 // output pixels first, then finish them, so that the residual / skip read latency overlaps.
 enum { EPI_PLAIN = 0, EPI_RES = 1, EPI_UP2 = 2 };
 

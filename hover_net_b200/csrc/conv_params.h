@@ -1,4 +1,4 @@
-// Parameter blocks shared by the CUDA-core referee convolution (conv_ref.cu) and the tcgen05
+// Parameter blocks shared by the CUDA-core referee convolution (conv_ref.cu) and the wgmma
 // convolution (conv_tc.cu).  Activations are NHWC.  A "split" tensor stores x as two fp16 planes
 // hi = fp16(x), lo = fp16(x - hi): x ~= hi + lo to ~2^-22 relative, which lets the tensor cores
 // reproduce fp32-grade products with three fp16 MMAs (hi*hi + hi*lo + lo*hi, fp32 accumulate).

@@ -1,6 +1,6 @@
-// CUDA-core kernels of the CNN path (sm_100a):
+// CUDA-core kernels of the CNN path (sm_90a):
 //   k_conv_ref   generic NHWC implicit-GEMM convolution in fp32 on split-fp16 operands.  It is the
-//                on-device referee for the tcgen05 kernel (same operands, same epilogue) and the
+//                on-device referee for the wgmma kernel (same operands, same epilogue) and the
 //                executor for layers the tensor-core kernel does not take.
 //   k_conv0      7x7x3 -> 64 stem on the uint8 image (reference net_desc.py:27-35,103,115)
 //   k_bnrelu     BatchNorm(eval)+ReLU raw fp32 -> split (dense-unit preact / blk_bna, net_utils.py:98-99,135-142)
@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(256) k_bnrelu(RawRef in, int B, const float *_
 void launch_bnrelu(const RawRef &in, int B, const float *scale, const float *shift, const SplitRef &out,
                    cudaStream_t s) {
     long long total = (long long)B * in.h * in.w * (in.c / 4);
-    int blocks = (int)std::min<long long>(cdiv(total, 256), 148 * 16);
+    int blocks = (int)std::min<long long>(cdiv(total, 256), 132 * 16);
     k_bnrelu<<<blocks, 256, 0, s>>>(in, B, scale, shift, out);
 }
 
@@ -296,7 +296,7 @@ __global__ void __launch_bounds__(256) k_up2_add(RawRef in, int B, SplitRef skip
 
 void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRef &out, cudaStream_t s) {
     long long total = (long long)B * 4 * in.h * in.w * (in.c / 8);
-    int blocks = (int)std::min<long long>(cdiv(total, 256), 148 * 32);
+    int blocks = (int)std::min<long long>(cdiv(total, 256), 132 * 32);
     k_up2_add<<<blocks, 256, 0, s>>>(in, B, skip, out);
 }
 

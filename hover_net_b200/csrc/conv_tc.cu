@@ -1,4 +1,4 @@
-// tcgen05 convolution for sm_100a: im2col-free NHWC implicit GEMM.
+// wgmma convolution for sm_90a (Hopper): im2col-free NHWC implicit GEMM.
 //
 //   D[pixel, cout] = sum_{tap} sum_{cin}  A_tap[pixel, cin] * W_tap[cout, cin]
 //
@@ -8,38 +8,26 @@
 //   addressing (out-of-bounds zero fill, elementStrides) -- no im2col buffer exists anywhere.
 //   1x1 stride-1 convolutions over a dense buffer use a flat 2-D [pixels, channels] map instead.
 // * W tiles (BLOCK_N couts x 64 cin, hi and lo) come from the [tap][cout][cin] K-major weight tensor.
-// * Both operands land in 128B-swizzled shared memory; one elected thread issues
-//   tcgen05.mma.cta_group::1.kind::f16 (M=128, K=16) twice per K-slice: a_hi x [w_hi | w_lo] (N = 2*BLOCK_N,
-//   the two weight tiles are adjacent in shared memory) and a_lo x w_hi (N = BLOCK_N); the epilogue sums the
-//   halves: hi*hi + hi*lo + lo*hi, fp32 accumulation => fp32-grade products from fp16 tensor cores.
-// * Persistent CTAs (one per SM), warp-specialised: warp0 = TMA producer, warp1 = MMA issuer (+TMEM
-//   allocator), warps 2..9 = epilogue (tcgen05.ld -> registers -> fused BN/ReLU/residual/upsample ->
-//   global).  Shared-memory ring of STAGES operand slots; two TMEM accumulation buffers so the epilogue
-//   of tile i overlaps the main loop of tile i+1.
-// * Accumulation precision: the tensor core adds into the fp32 accumulator with truncation, a bias
-//   that grows with the number of MMAs chained into one accumulator (measured on B200: ~4e-5
-//   relative at K=9216).  The K loop is therefore cut into segments of 4 64-channel slices (32 MMA
-//   instructions); each segment accumulates in its own TMEM buffer and the epilogue warps drain it into
-//   fp32 registers (round-to-nearest adds) while the next segment runs in the other buffer.
-// * XF variant (1x1 layers fed by a raw fp32 tensor through a pre-activation BatchNorm+ReLU): four
+// * Both operands land in 128B-swizzled shared memory and are read from there by wgmma (both K-major).  Per K=16 step
+//   three m64nNk16 instructions accumulate a_hi*w_hi + a_hi*w_lo + a_lo*w_hi in fp32 registers: fp32-grade products
+//   from fp16 tensor cores.
+// * Persistent CTAs (one per SM), warp-specialised: warp 0 = TMA producer; warpgroups 1 and 2 = consumers, each issuing
+//   the wgmma of 64 of the tile's 128 pixel rows over all BLOCK_N columns and running the fused epilogue (BN/ReLU/
+//   residual/upsample -> global) straight from its accumulator fragment.  A shared-memory ring of STAGES operand slots
+//   lets the producer run ahead, also across the consumers' epilogue.
+// * Accumulation precision: the K loop is cut into segments of G.seg 64-channel slices; each segment accumulates in the
+//   wgmma registers from zero and is then added into a separate fp32 sum with round-to-nearest adds, so the number of
+//   products chained inside the tensor core stays bounded however large K is.
+// * XF variant (1x1 layers fed by a raw fp32 tensor through a pre-activation BatchNorm+ReLU): three
 //   extra "transform" warps build the A tiles themselves -- coalesced fp32 loads, y=relu(x*scale+shift),
 //   fp16 hi/lo split, 128B-swizzled st.shared, fence.proxy.async -- so the pre-activated copy of the
 //   tensor never exists in HBM (no separate BN/ReLU pass, no second output of the producing layer).
-// * HALO variant (k x k stride-1 layers): the per-tap path re-fetches the A tile once per filter tap, which
-//   puts thin layers (cout 32/64) at the chip-wide L2->SM cap (~6300 B/clk, ncu: 11.2 TB/s).  Here ONE halo tile
-//   ((16+kh-1) x (8+kw-1) pixels x 64 channels, hi and lo) is fetched per 64-channel block and every tap's
-//   MMA reads its shifted 16x8 window straight out of it: the A descriptor starts (ky*Wp + kx) rows into the
-//   halo and steps SBO = Wp*128 B between 8-pixel rows.  tcgen05.mma resolves the 128B swizzle from absolute
-//   shared-memory address bits (tools/umma_shift_probe.cu, measured on B200: any 128 B-row start offset and
-//   any SBO multiple of 128 B reads what TMA wrote), so no re-layout is needed.  Weights stream through their
-//   own ring, one (tap, 64-channel) tile per stage.
-// * Two specialised sibling kernels further down: k_conv_ar (1x1 + fp32 residual with the A tile resident in shared
-//   memory while the unit's weight tiles stream; residual added in place in swizzled per-warp regions) and k_conv_rs
-//   (the decoder's grouped k x k layers: the kw taps of a filter row stacked along N, col2im in the epilogue).
 // * Flat (2-D map) operands streamed from HBM get a cp.async.bulk.prefetch.tensor L2 cursor a few K-slices ahead.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cstring>
 #include <mutex>
 
 #include "common.cuh"
@@ -84,119 +72,162 @@ __device__ __forceinline__ void tma_4d(uint32_t dst, const void *tmap, uint32_t 
                  ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 // L2 prefetch of a tensor-map box: no shared memory, no barrier -- used to run several K-slices ahead of the loads on
-// operands that come from HBM (the rings below hold 2-3 slices, less than one DRAM round trip under load)
+// operands that come from HBM (the rings below hold 2-4 slices, less than one DRAM round trip under load)
 __device__ __forceinline__ void tma_prefetch_2d(const void *tmap, int c0, int c1) {
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused (=1).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t sbo = 1024) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R> __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// K-major, 128B-swizzled operand tile (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): rows of 128 B, 8-row
+// groups 1024 B apart (SBO), LBO unused for swizzled K-major layouts.  Tiles start 1024-aligned, so the base offset is 0;
+// the K=16 steps inside a 64-channel slice advance the start address by 32 B (the swizzle is applied to address bits).
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
     d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(sbo >> 4) << 32;
-    d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;   // SWIZZLE_128B
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;   // SWIZZLE_128B
     return d;
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, fp32 accumulators in registers.
+// Fragment: register 4j + 2h + e holds row (warp & 3) * 16 + lane / 4 + 8h, column 8j + 2 (lane % 4) + e.
+template <int N> struct Wgmma;
+#define HVN_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define HVN_WGMMA(N, R, DREGS, P, AB, ...)                                                                             \
+    template <> struct Wgmma<N> {                                                                                      \
+        static __device__ __forceinline__ void mma(float (&d)[R], uint64_t a, uint64_t b, uint32_t accum) {            \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\twgmma.mma_async.sync.aligned.m64n" #N      \
+                         "k16.f32.f16.f16 {" DREGS "}, " AB ", p, 1, 1, 0, 0;\n\t}"                                    \
+                         : __VA_ARGS__ : "l"(a), "l"(b), "r"(accum));                                                  \
+        }                                                                                                              \
+    };
+HVN_WGMMA(32, 16, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15", "%18", "%16, %17", HVN_F8(0), HVN_F8(8))
+HVN_WGMMA(64, 32, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31", "%34", "%32, %33", HVN_F8(0), HVN_F8(8), HVN_F8(16), HVN_F8(24))
+HVN_WGMMA(128, 64, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63", "%66", "%64, %65", HVN_F8(0), HVN_F8(8), HVN_F8(16), HVN_F8(24), HVN_F8(32), HVN_F8(40), HVN_F8(48), HVN_F8(56))
+#undef HVN_WGMMA
+#undef HVN_F8
+
+// One 64-channel K-slice of the split product: a_hi*w_hi + a_hi*w_lo + a_lo*w_hi (4 K=16 steps, +32 B each)
+template <int N>
+__device__ __forceinline__ void mma_slice(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, bool zero) {
+    const uint64_t dah = wg_desc(a_hi), dal = wg_desc(a_lo), dbh = wg_desc(b_hi), dbl = wg_desc(b_lo);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t ko = (uint64_t)(2 * k);
+        Wgmma<N>::mma(d, dah + ko, dbh + ko, (zero && k == 0) ? 0u : 1u);
+        Wgmma<N>::mma(d, dah + ko, dbl + ko, 1u);
+        Wgmma<N>::mma(d, dal + ko, dbh + ko, 1u);
+    }
 }
 
 struct TcGeom {
     int flat, bw, bh, tiles_x, tiles_y, tiles_m, tiles_n, kchunks, seg;
     int k1;  // > 0: K-slices [0,k1) come from the first source, [k1,kchunks) from the second (fused shortcut)
     long long m_total;
-    // HALO variant: halo tile of halo_w x halo_h pixels per 64-channel block, a_plane bytes per fp16 plane
-    // (1024-aligned), na slots (1 or 2)
-    int halo_w, halo_h, a_plane, na;
     int pf;        // flat (2-D map) operands: L2 prefetch distance in K-slices (0 = off)
-    int lean_epi;  // write-out with per-tile precomputed output offsets (plain / residual epilogues)
-    int xf_early;  // XF: raw slot released right after its values are in registers, raw loads one slice ahead of the W wait
     int xf_trunc;  // XF transform: truncating hi/lo split (split4_relu_trunc) instead of the round-to-nearest one
 };
 
-constexpr int SMEM_LIMIT = 232448;       // opt-in dynamic shared memory per CTA (227 KB)
-constexpr int TC_THREADS = 320;          // warp0 TMA, warp1 MMA, warps 2..9 epilogue
-// XF variant: warps 10.. transform the A operand.  The transform (~7.5 instructions per element, 500 per thread and
-// K-slice with four warps) runs about as long as the K-slice's MMAs, so its warp count sets the layer's speed: six warps
-// behind a BLOCK_N = 128 tile (512 threads: the 128 registers per thread its epilogue needs are still available), eight
-// behind a BLOCK_N = 64 tile, whose K-slice leaves the tensor core in 570 instead of 800 cycles.
-template <int BLOCK_N> constexpr int xf_warps() { return BLOCK_N >= 128 ? 6 : 8; }
-constexpr int EP_WARPS = 8;
+constexpr int SMEM_LIMIT = 232448;       // opt-in dynamic shared memory per CTA on sm_90 (227 KB)
+constexpr int TC_THREADS = 384;          // warpgroup 0: TMA producer (warp 0) + XF transform (warps 1..3); warpgroups 1, 2: wgmma
+constexpr int XF_WARPS = 3;
+constexpr int CONS_WARPS = 8;
 constexpr int A_TILE_BYTES = 128 * 128;  // 128 rows x 64 fp16
+constexpr uint32_t RAW_TILE_BYTES = 128 * 64 * 4;
 
 template <int BLOCK_N> __host__ __device__ constexpr int tc_stage_bytes() { return 2 * A_TILE_BYTES + 2 * BLOCK_N * 128; }
+template <int BLOCK_N, int STAGES, bool XF> constexpr int tc_smem() {
+    return 1024 + STAGES * tc_stage_bytes<BLOCK_N>() + (XF ? 2 * (int)RAW_TILE_BYTES : 0) + 8 * (2 * STAGES + 4);
+}
 
-// RT (residual mode, BLOCK_N = 64): the fp32 residual tile [128 px][64 ch] is fetched by TMA into a
-// two-slot shared-memory ring one tile ahead (tm_a2_hi carries its tensor map), instead of by
-// per-thread global loads -- the thin residual layers are bound by how many bytes an SM keeps in flight.
-template <int BLOCK_N, int STAGES, int MODE, bool XF, bool RT = false, bool HALO = false>
-__global__ void __launch_bounds__(TC_THREADS + (XF ? xf_warps<BLOCK_N>() * 32 : 0), 1)
+// Output element offsets of one accumulator row (pixel); -1 = no such pixel.
+struct PixOff {
+    long long res = -1, raw = -1, spl = -1, skip = -1;
+};
+
+template <int MODE>
+__device__ __forceinline__ PixOff pix_offsets(const ConvParams &P, bool valid, int n, int oy, int ox) {
+    PixOff o;
+    if (!valid) return o;
+    if (MODE == EPI_RES) o.res = n * P.res.sN + (long long)oy * P.res.sH + (long long)ox * P.res.sW;
+    if (P.out_raw.p) o.raw = n * P.out_raw.sN + (long long)oy * P.out_raw.sH + (long long)ox * P.out_raw.sW;
+    if (MODE == EPI_UP2) {
+        o.spl = n * P.out_split.sN + (long long)(2 * oy) * P.out_split.sH + (long long)(2 * ox) * P.out_split.sW;
+        o.skip = n * P.skip.sN + (long long)(2 * oy) * P.skip.sH + (long long)(2 * ox) * P.skip.sW;
+    } else if (P.out_split.hi) {
+        o.spl = n * P.out_split.sN + (long long)oy * P.out_split.sH + (long long)ox * P.out_split.sW;
+    }
+    return o;
+}
+
+__device__ __forceinline__ void store_split2(const SplitRef &o, long long off, float a, float b) {
+    __half h0, l0, h1, l1;
+    split_f32(a, h0, l0, o.flag);
+    split_f32(b, h1, l1, o.flag);
+    *reinterpret_cast<__half2 *>(o.hi + off) = __halves2half2(h0, h1);
+    *reinterpret_cast<__half2 *>(o.lo + off) = __halves2half2(l0, l1);
+}
+
+// Channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  Same operations, in the same order, as
+// epi_finish (conv_epilogue.cuh) on four channels.
+template <int MODE>
+__device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, float2 s, float2 b) {
+    if constexpr (MODE == EPI_RES) {
+        const float2 r = *reinterpret_cast<const float2 *>(P.res.p + o.res + c);
+        v0 += r.x; v1 += r.y;
+    }
+    if (o.raw >= 0) *reinterpret_cast<float2 *>(P.out_raw.p + o.raw + c) = make_float2(v0, v1);
+    if constexpr (MODE == EPI_UP2) {
+#pragma unroll
+        for (int d = 0; d < 4; ++d) {
+            const long long so = o.skip + (d >> 1) * P.skip.sH + (d & 1) * P.skip.sW + c;
+            const __half2 sh = *reinterpret_cast<const __half2 *>(P.skip.hi + so);
+            const __half2 sl = *reinterpret_cast<const __half2 *>(P.skip.lo + so);
+            store_split2(P.out_split, o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c,
+                         v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
+        }
+    } else if (o.spl >= 0) {
+        float t0 = v0, t1 = v1;
+        if (P.scale) { t0 = t0 * s.x + b.x; t1 = t1 * s.y + b.y; }
+        if (P.relu) { t0 = fmaxf(t0, 0.f); t1 = fmaxf(t1, 0.f); }
+        store_split2(P.out_split, o.spl + c, t0, t1);
+    }
+}
+
+template <int BLOCK_N, int STAGES, int MODE, bool XF>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
           const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
           const __grid_constant__ CUtensorMap tm_a2_hi, const __grid_constant__ CUtensorMap tm_a2_lo,
           const ConvParams P, const TcGeom G) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // HALO: the ring holds weight tiles only; the halo slots live where XF/RT keep their staging ring
-    constexpr int STAGE_BYTES = HALO ? 2 * BLOCK_N * 128 : tc_stage_bytes<BLOCK_N>();
+    constexpr int STAGE_BYTES = tc_stage_bytes<BLOCK_N>();
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
-    // barriers: full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2]; then the TMEM base pointer
+    const uint32_t raw_base = smem_base + STAGES * STAGE_BYTES;             // XF: 2-slot ring of raw fp32 [128][64] tiles
+    const uint32_t bar_base = raw_base + (XF ? 2 * RAW_TILE_BYTES : 0u);
+    // barriers: full[STAGES], empty[STAGES], raw_full[2], raw_empty[2]
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    // XF only: raw_full[2], raw_empty[2] barriers and a 2-slot ring of raw fp32 [128][64] staging tiles
-    auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + 4) + 16u + 8u * r; };
-    auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + 4) + 16u + 8u * (2 + r); };
-    const uint32_t ep_base = bar_base + 8u * (2 * STAGES + 4) + 48u;  // 8 warps x [32][32] fp32 transpose tiles (XOR-swizzled)
-    const uint32_t raw_base = (ep_base + EP_WARPS * 4096u + 1023u) & ~1023u;
-    constexpr uint32_t RAW_TILE_BYTES = 128 * 64 * 4;
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+    auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + r); };
+    auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + 2 + r); };
 
-    constexpr int XF_WARPS = xf_warps<BLOCK_N>();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // two accumulation buffers of 2*BLOCK_N columns: [hi*hi + lo*hi | hi*lo] (see the MMA issuer)
-    constexpr uint32_t TMEM_COLS = 4 * BLOCK_N;
-
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), XF ? 1 + XF_WARPS : 1); mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), BLOCK_N >= 64 ? 256 : 128); }
-        if (XF || RT) for (int r = 0; r < 2; ++r) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), XF ? XF_WARPS : EP_WARPS); }
-        if (HALO) for (int r = 0; r < 2; ++r) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), 1); }  // halo slots: full / empty
+    // warp index broadcast from lane 0: provably warp-uniform, so the role branches below do not count as divergent
+    // paths around the wgmma (ptxas would otherwise serialise them)
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), XF ? 1 + XF_WARPS : 1); mbar_init(empty_bar(s), CONS_WARPS); }
+        if (XF) for (int r = 0; r < 2; ++r) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), XF_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     const int total_tiles = G.tiles_m * G.tiles_n;
     const int taps = P.w.taps;
@@ -206,54 +237,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
     if (warp == 0) {
         // ===================== TMA producer =====================
         if (lane == 0) {
-          if constexpr (HALO) {
-            // Blocks = (tile, 64-channel slice) pairs in execution order.  The halo of block b+1 is requested
-            // while block b's weight tiles stream, so its latency hides behind a block's worth of MMAs.
-            const uint32_t halo_tx = (uint32_t)(2 * G.halo_w * G.halo_h * 128);
-            auto issue_halo = [&](int tile, int kc, int ablk) {
-                const int tm = tile / G.tiles_n;
-                const int per_img = G.tiles_x * G.tiles_y;
-                const int n_img = tm / per_img;
-                const int r = tm - n_img * per_img;
-                const int y0 = (r / G.tiles_x) * G.bh, x0 = (r - (r / G.tiles_x) * G.tiles_x) * G.bw;
-                const int slot = ablk % G.na;
-                const uint32_t ph = (uint32_t)(ablk / G.na) & 1u;
-                mbar_wait(rempty_bar(slot), ph ^ 1u);
-                mbar_expect_tx(rfull_bar(slot), halo_tx);
-                const uint32_t dst = raw_base + (uint32_t)(slot * 2 * G.a_plane);
-                tma_4d(dst, &tm_a_hi, rfull_bar(slot), kc * 64, x0 - P.pad_l, y0 - P.pad_t, n_img);
-                tma_4d(dst + (uint32_t)G.a_plane, &tm_a_lo, rfull_bar(slot), kc * 64, x0 - P.pad_l, y0 - P.pad_t, n_img);
-            };
-            int ablk = 0, wit = 0;
-            // After this tap's weights the next halo is requested.  Two slots: as soon as the ring has wrapped
-            // once (the previous block is then complete); one slot: only after ALL of this block's weights are
-            // in flight -- the request waits for this block's MMAs, which need those weights.
-            const int t_next = G.na >= 2 ? (taps < STAGES ? taps : STAGES) - 1 : taps - 1;
-            if ((int)blockIdx.x < total_tiles) issue_halo(blockIdx.x, 0, 0);
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int tn = tile - (tile / G.tiles_n) * G.tiles_n;
-                for (int kc = 0; kc < G.kchunks; ++kc, ++ablk) {
-                    for (int tap = 0; tap < taps; ++tap, ++wit) {
-                        const int s = wit % STAGES;
-                        const uint32_t ph = (uint32_t)(wit / STAGES) & 1u;
-                        mbar_wait(empty_bar(s), ph ^ 1u);
-                        const uint32_t b_hi = smem_base + s * STAGE_BYTES, b_lo = b_hi + BLOCK_N * 128;
-                        mbar_expect_tx(full_bar(s), (uint32_t)(2 * BLOCK_N * 128));
-                        tma_3d(b_hi, &tm_w_hi, full_bar(s), kc * 64, tn * BLOCK_N, tap);
-                        tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
-                        if (tap == t_next) {
-                            if (kc + 1 < G.kchunks) issue_halo(tile, kc + 1, ablk + 1);
-                            else if (tile + (int)gridDim.x < total_tiles) issue_halo(tile + gridDim.x, 0, ablk + 1);
-                        }
-                    }
-                }
-            }
-          } else {
             int it_global = 0;
-            int tile_count = 0;
             // L2 prefetch cursor, G.pf K-slices ahead of the loads through the same (tile, slice) sequence.  Flat layers
-            // only: their A operand is a whole encoder tensor streamed from HBM (571 MB for d1's running sum at 16
-            // patches); with a 2-slot raw ring the XF layers ran at one DRAM round trip per two K-slices.
+            // only: their A operand is a whole encoder tensor streamed from HBM.
             const bool pf_on = G.flat && G.pf > 0;
             int pf_tile = blockIdx.x, pf_it = 0;
             auto pf_step = [&]() {
@@ -270,28 +256,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 if (++pf_it == kiters) { pf_it = 0; pf_tile += gridDim.x; }
             };
             if (pf_on) for (int i = 0; i < G.pf; ++i) pf_step();
-            // XF, G.xf_early: the raw fp32 tile of K-slice i+1 is requested BEFORE this thread blocks on the operand stage of
-            // slice i (whose release needs the MMAs of slice i-2) -- its own cursor through the (tile, slice) sequence.
-            // Together with the transform warps handing the raw slot back as soon as its values are in registers, a raw
-            // slot cycles in (load latency + LDS) instead of (load latency + stage wait + transform).
-            int rw_tile = blockIdx.x, rw_it = 0, rw_count = 0;
-            auto raw_step = [&]() {
-                if (rw_tile >= total_tiles) return;
-                const int tmr = rw_tile / G.tiles_n;
-                const int r = rw_count & 1;
-                mbar_wait(rempty_bar(r), (((uint32_t)(rw_count >> 1)) & 1u) ^ 1u);
-                mbar_expect_tx(rfull_bar(r), (uint32_t)((G.flat ? 128 : G.bw * G.bh) * 256));
-                if (G.flat) tma_2d(raw_base + r * RAW_TILE_BYTES, &tm_a_hi, rfull_bar(r), rw_it * 64, tmr * 128);
-                else {
-                    const int per_img = G.tiles_x * G.tiles_y;
-                    const int ni = tmr / per_img, rr = tmr - ni * per_img;
-                    tma_4d(raw_base + r * RAW_TILE_BYTES, &tm_a_hi, rfull_bar(r), rw_it * 64, (rr - (rr / G.tiles_x) * G.tiles_x) * G.bw,
-                           (rr / G.tiles_x) * G.bh, ni);
-                }
-                ++rw_count;
-                if (++rw_it == kiters) { rw_it = 0; rw_tile += gridDim.x; }
-            };
-            if (XF && G.xf_early) raw_step();
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int tm = tile / G.tiles_n, tn = tile - tm * G.tiles_n;
                 int n_img = 0, y0 = 0, x0 = 0;
@@ -304,25 +268,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                     y0 = (r / G.tiles_x) * G.bh;
                     x0 = (r - (r / G.tiles_x) * G.tiles_x) * G.bw;
                 }
-                if constexpr (RT) {  // residual tile of this output tile -> ring slot (flat 2-D map [channels, pixels])
-                    const int r = tile_count & 1;
-                    const uint32_t rph = (uint32_t)(tile_count >> 1) & 1u;
-                    mbar_wait(rempty_bar(r), rph ^ 1u);
-                    mbar_expect_tx(rfull_bar(r), RAW_TILE_BYTES);
-                    tma_2d(raw_base + r * RAW_TILE_BYTES, &tm_a2_hi, rfull_bar(r), tn * BLOCK_N, (int)m0);
-                    ++tile_count;
-                    if (G.pf > 0) {  // residual of the tile after next -> L2 (the ring itself holds one tile of look-ahead)
-                        const int t2 = tile + 2 * (int)gridDim.x;
-                        if (t2 < total_tiles) tma_prefetch_2d(&tm_a2_hi, (t2 % G.tiles_n) * BLOCK_N, (t2 / G.tiles_n) * 128);
-                    }
-                }
                 for (int it = 0; it < kiters; ++it, ++it_global) {
                     if (pf_on) pf_step();
-                    if (XF && G.xf_early) raw_step();   // slice it_global + 1
-                    else if constexpr (XF) {
-                        // raw fp32 A tile of this K-slice -> staging ring (tm_a_hi is the fp32 map).  Issued BEFORE the
-                        // wait for the operand stage: the raw slot frees up a whole transform earlier than the stage does,
-                        // and a raw load that waits for the stage costs the XF layers 15 % (measured, r2d vs r2a)
+                    if constexpr (XF) {
+                        // raw fp32 A tile of this K-slice -> staging ring (tm_a_hi is the fp32 map).  Issued before the
+                        // wait for the operand stage: the raw slot frees up a whole transform earlier than the stage does.
                         const int r = it_global & 1;
                         const uint32_t rph = (uint32_t)(it_global >> 1) & 1u;
                         mbar_wait(rempty_bar(r), rph ^ 1u);
@@ -366,104 +316,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                     tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
                 }
             }
-          }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            // instruction descriptor: D=f32, A=B=f16, both K-major, N>>3 at bit 17, M>>4 at bit 24
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(BLOCK_N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            // Measured on B200 (tools/umma_rate_probe.cu): an SS-mode M=128 K=16 MMA costs max(71.6, N/2) cycles --
-            // the 128x32 B A-operand read is a floor that N <= 128 never amortises.  The W hi and lo tiles are
-            // adjacent in shared memory, so ONE N = 2*BLOCK_N instruction computes a_hi*[w_hi | w_lo] into the two
-            // halves of the accumulation buffer, and a second N = BLOCK_N instruction adds a_lo*w_hi to the first
-            // half: 2 instructions per K-step instead of 3; the epilogue sums the halves in fp32 registers.
-            const uint32_t idesc2 = (1u << 4) | ((uint32_t)(2 * BLOCK_N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-          if constexpr (HALO) {
-            // it = kc * taps + tap (channel-slice major): all taps of a slice read the same halo slot.
-            // This one thread paces the tensor core, so its per-tap instruction count matters (measured: with two
-            // integer divisions and three descriptor builds per tap it issued 8 MMAs per ~1100 cycles, half the
-            // tensor core's rate): every index is carried incrementally and a descriptor is its constant upper
-            // part plus (address >> 4).
-            const uint32_t sbo = (uint32_t)G.halo_w * 128u;
-            const uint64_t adesc0 = umma_desc(0, sbo), bdesc0 = umma_desc(0);
-            const uint32_t a_lo_off = (uint32_t)G.a_plane >> 4;
-            int scount = 0;
-            uint32_t ws = 0, wph = 0;       // weight ring stage / phase
-            uint32_t slot = 0, aph_h = 0;   // halo slot / phase
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                int tap = 0, ky = 0, kx = 0;
-                for (int it0 = 0; it0 < kiters; it0 += G.seg, ++scount) {
-                    const int as = scount & 1;
-                    const uint32_t aph = (uint32_t)(scount >> 1) & 1u;
-                    mbar_wait(tempty_bar(as), aph ^ 1u);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(as * 2 * BLOCK_N);
-                    const int it1 = min(it0 + G.seg, kiters);
-                    for (int it = it0; it < it1; ++it) {
-                        if (tap == 0) mbar_wait(rfull_bar(slot), aph_h);
-                        mbar_wait(full_bar(ws), wph);
-                        tc_fence_after();
-                        const uint32_t a0 = raw_base + slot * (uint32_t)(2 * G.a_plane) + (uint32_t)((ky * G.halo_w + kx) * 128);
-                        const uint64_t da_hi = adesc0 + (uint64_t)((a0 & 0x3FFFFu) >> 4), da_lo = da_hi + a_lo_off,
-                                       db_hi = bdesc0 + (uint64_t)(((smem_base + ws * STAGE_BYTES) & 0x3FFFFu) >> 4);  // [w_hi | w_lo]
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t ko = (uint64_t)(2 * k);
-                            tc_mma_f16(d_tmem, da_hi + ko, db_hi + ko, idesc2, (it > it0 || k > 0) ? 1u : 0u);
-                            tc_mma_f16(d_tmem, da_lo + ko, db_hi + ko, idesc, 1u);
-                        }
-                        tc_commit(empty_bar(ws));
-                        if (++ws == (uint32_t)STAGES) { ws = 0; wph ^= 1u; }
-                        if (++kx == P.w.kw) { kx = 0; ++ky; }
-                        if (++tap == taps) {  // last tap of this channel slice: the halo slot is reusable
-                            tc_commit(rempty_bar(slot));
-                            tap = 0; ky = 0; kx = 0;
-                            if (++slot == (uint32_t)G.na) { slot = 0; aph_h ^= 1u; }
-                        }
-                    }
-                    tc_commit(tfull_bar(as));
-                }
-            }
-          } else {
-            int it_global = 0, scount = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                for (int it0 = 0; it0 < kiters; it0 += G.seg, ++scount) {
-                    const int as = scount & 1;
-                    const uint32_t aph = (uint32_t)(scount >> 1) & 1u;
-                    mbar_wait(tempty_bar(as), aph ^ 1u);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(as * 2 * BLOCK_N);
-                    const int it1 = min(it0 + G.seg, kiters);
-                    for (int it = it0; it < it1; ++it, ++it_global) {
-                        const int s = it_global % STAGES;
-                        const uint32_t ph = (uint32_t)(it_global / STAGES) & 1u;
-                        mbar_wait(full_bar(s), ph);
-                        tc_fence_after();
-                        const uint32_t sa = smem_base + s * STAGE_BYTES;
-                        const uint64_t da_hi = umma_desc(sa), da_lo = umma_desc(sa + A_TILE_BYTES),
-                                       db_hi = umma_desc(sa + 2 * A_TILE_BYTES);  // [w_hi | w_lo]: 2*BLOCK_N contiguous rows
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {  // 4 x K=16 inside the 64-channel slice: +32 B per step
-                            const uint64_t ko = (uint64_t)(2 * k);
-                            tc_mma_f16(d_tmem, da_hi + ko, db_hi + ko, idesc2, (it > it0 || k > 0) ? 1u : 0u);
-                            tc_mma_f16(d_tmem, da_lo + ko, db_hi + ko, idesc, 1u);
-                        }
-                        tc_commit(empty_bar(s));  // slot reusable once these MMAs have read it
-                    }
-                    tc_commit(tfull_bar(as));     // segment complete -> epilogue warps drain it
-                }
-            }
-          }
-        }
-    } else if (XF && warp >= 2 + EP_WARPS) {
-        // ===================== A-operand transform (warps 10..17, XF only) =====================
+    } else if (XF && warp < 4) {
+        // ===================== A-operand transform (warps 1..3, XF only) =====================
         // thread -> (row group rg = t>>4, float4 column l16 = t&15), rows rg + 16*i: raw fp32 staging tile
         // (row-major [128][64], filled by TMA) -> y = relu(x*scale+shift) -> fp16 hi/lo -> swizzled A tiles.
-        // All eight row loads of a K-slice are issued before the first value is used: the loop used to be one
-        // LDS -> 30-instruction dependent chain -> STS per row (ncu/SASS: no two loads in flight), which paced the
-        // tensor core at roughly half its rate on every pre-activation 1x1 layer.
-        const int t = threadIdx.x - (2 + EP_WARPS) * 32;
+        // All row loads of a K-slice are issued before the first value is used.
+        const int t = threadIdx.x - 32;
         const int l16 = t & 15, rg = t >> 4;
         const int wl = t & 31;
         constexpr int RG = XF_WARPS * 2;              // row groups: rows rg, rg + RG, ...
@@ -492,17 +351,14 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 float4 v[XR];
 #pragma unroll
                 for (int i = 0; i < XR; ++i)  // rows TMA did not write read as 0: finite, and invisible to the range guard
-                    v[i] = rg + RG * i < vrows ? *reinterpret_cast<const float4 *>(src + i * RG * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    v[i] = rg + RG * i < min(vrows, 128) ? *reinterpret_cast<const float4 *>(src + i * RG * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
                 // y = x*scale + shift in place: in-order issue puts every instruction below behind the completed LDS of
-                // this lane, so the raw slot can go back to the producer NOW (G.xf_early) -- a whole stage wait + split +
-                // store phase before the old hand-back at the end of the slice
+                // this lane, so the raw slot can go back to the producer now
 #pragma unroll
                 for (int i = 0; i < XR; ++i)
                     v[i] = make_float4(fmaf(v[i].x, sc.x, sh.x), fmaf(v[i].y, sc.y, sh.y), fmaf(v[i].z, sc.z, sh.z), fmaf(v[i].w, sc.w, sh.w));
-                if (G.xf_early) {
-                    __syncwarp();
-                    if (wl == 0) mbar_arrive(rempty_bar(r));
-                }
+                __syncwarp();
+                if (wl == 0) mbar_arrive(rempty_bar(r));
                 mbar_wait(empty_bar(s), ph ^ 1u);
                 uint8_t *a_hi = smem_gen + s * STAGE_BYTES, *a_lo = a_hi + A_TILE_BYTES;
                 // range guard: running maximum, tested once per tile (a flag store inside this loop cost the XF layers
@@ -534,618 +390,90 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                         *reinterpret_cast<uint2 *>(a_lo + off) = ol;
                     }
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> visible to the MMA (async proxy)
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> visible to wgmma (async proxy)
                 __syncwarp();
-                if (wl == 0) { mbar_arrive(full_bar(s)); if (!G.xf_early) mbar_arrive(rempty_bar(r)); }
+                if (wl == 0) mbar_arrive(full_bar(s));
             }
             if (rmax > 65504.f && P.a.flag) *P.a.flag = 1u;
         }
-    } else {
-        // ===================== epilogue (warps 2..9) =====================
-        // warps w and w+4 share a TMEM lane quadrant (w & 3) and split the tile's columns in halves
-        constexpr int CW = BLOCK_N >= 64 ? BLOCK_N / 2 : BLOCK_N;  // columns per epilogue warp
-        const int quad = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int row = quad * 32 + lane;     // accumulator row == pixel index inside the tile
-        if (BLOCK_N >= 64 || half == 0) {
-        const int cb = half * CW;
-        float *ep_tile = reinterpret_cast<float *>(smem_raw + (ep_base - smem_u32(smem_raw))) + (warp - 2) * 32 * 32;
-        int scount = 0;
-        int tcount_e = 0;
+    } else if (warp >= 4) {
+        // ===================== wgmma consumers (warpgroups 1, 2) =====================
+        const int wg = (warp >> 2) - 1;                     // rows [64 wg, 64 wg + 64) of the tile
+        const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows ra and ra + 8
+        constexpr int NR = BLOCK_N / 2;
+        float acc[NR], sum[NR];
+#pragma unroll
+        for (int j = 0; j < NR; ++j) acc[j] = 0.f;
+        auto release = [&](int s) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));
+        };
+        int it_global = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int tm = tile / G.tiles_n, tn = tile - tm * G.tiles_n;
-            bool valid;
-            int n_img, oy, ox;
-            if (G.flat) {
-                long long m = (long long)tm * 128 + row;
-                valid = m < G.m_total;
-                long long hw = (long long)P.ho * P.wo;
-                n_img = valid ? (int)(m / hw) : 0;
-                int r = valid ? (int)(m - (long long)n_img * hw) : 0;
-                oy = r / P.wo; ox = r - oy * P.wo;
-            } else {
-                const int per_img = G.tiles_x * G.tiles_y;
-                n_img = tm / per_img;
-                const int r = tm - n_img * per_img;
-                const int ty = r / G.tiles_x, tx = r - ty * G.tiles_x;
-                const int py = row / G.bw, px = row - py * G.bw;
-                oy = ty * G.bh + py; ox = tx * G.bw + px;
-                valid = row < G.bw * G.bh && oy < P.ho && ox < P.wo;
-            }
-            // The transposed write-out below maps lane -> (pixel sub_px + 4*it, channel group sub_g).  In
-            // residual mode the whole tile's residual values are requested now, before the accumulator is
-            // waited for, so their HBM latency hides behind the main loop.
-            const int sub_px = lane >> 3, sub_g = lane & 7;
-            constexpr int NCH = CW / 32;
-            constexpr bool REG_RES = MODE == EPI_RES && !RT;
-            float4 rpre[REG_RES ? NCH : 1][REG_RES ? 8 : 1];
-            if constexpr (REG_RES) {
 #pragma unroll
-                for (int it = 0; it < 8; ++it) {
-                    const int src = it * 4 + sub_px;
-                    const int pv = __shfl_sync(0xffffffffu, (int)valid, src);
-                    const int pn = __shfl_sync(0xffffffffu, n_img, src);
-                    const int py = __shfl_sync(0xffffffffu, oy, src);
-                    const int px = __shfl_sync(0xffffffffu, ox, src);
+            for (int j = 0; j < NR; ++j) sum[j] = 0.f;
+            int pend = -1;   // stage whose wgmma group may still be reading it
+            for (int it = 0; it < kiters; ++it, ++it_global) {
+                const int s = it_global % STAGES;
+                mbar_wait(full_bar(s), (uint32_t)(it_global / STAGES) & 1u);
+                const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;
+                const uint32_t sb = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES;
+                wg_fence();
+                mma_slice<BLOCK_N>(acc, sa, sa + A_TILE_BYTES, sb, sb + BLOCK_N * 128, it % G.seg == 0);
+                wg_commit();
+                if ((it + 1) % G.seg == 0 || it + 1 == kiters) {   // segment complete: drain it into the fp32 sum
+                    wg_wait<0>();
+                    wg_fence_regs(acc);
+                    if (pend >= 0) release(pend);
+                    release(s);
+                    pend = -1;
 #pragma unroll
-                    for (int cc = 0; cc < NCH; ++cc) {
-                        rpre[cc][it] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (pv)
-                            rpre[cc][it] = *reinterpret_cast<const float4 *>(
-                                P.res.p + pn * P.res.sN + (long long)py * P.res.sH + (long long)px * P.res.sW +
-                                tn * BLOCK_N + cb + cc * 32 + sub_g * 4);
-                    }
+                    for (int j = 0; j < NR; ++j) sum[j] += acc[j];
+                } else {
+                    wg_wait<1>();                                  // the previous slice's group is done with its stage
+                    if (pend >= 0) release(pend);
+                    pend = s;
                 }
             }
-            // Element offsets of this lane's pixel in the two outputs (-1 = no such output / no such pixel), computed ONCE per
-            // tile and shuffled to the write-out mapping below.  The write-out used to rebuild n*sN + oy*sH + ox*sW in
-            // 64-bit arithmetic for every (pixel, 32-channel block) behind four shuffles: half of its 1 878 instructions per
-            // 128 x 128 tile (SASS), and that loop paces every split-output layer with few K-slices (decoder conv1 layers:
-            // 12 k cycles per tile against 1 600 of MMA).
-            long long off_s = -1, off_r = -1;
-            if (MODE != EPI_UP2 && valid) {
-                if (P.out_split.hi) off_s = n_img * P.out_split.sN + (long long)oy * P.out_split.sH + (long long)ox * P.out_split.sW;
-                if (P.out_raw.p) off_r = n_img * P.out_raw.sN + (long long)oy * P.out_raw.sH + (long long)ox * P.out_raw.sW;
-            }
-            // BN scale / shift of this lane's 4 channels per 32-channel block: requested before the accumulator wait
-            float4 esc[NCH], esh[NCH], ews[NCH];
+            // ---- epilogue straight from the fragment: rows ra, ra + 8; two consecutive channels per register pair
+            PixOff po[2];
 #pragma unroll
-            for (int cc = 0; cc < NCH; ++cc) {
-                esc[cc] = make_float4(1.f, 1.f, 1.f, 1.f); esh[cc] = make_float4(0.f, 0.f, 0.f, 0.f);
-                ews[cc] = *reinterpret_cast<const float4 *>(P.w.oscale + tn * BLOCK_N + cb + cc * 32 + sub_g * 4);
-                if (MODE != EPI_UP2 && P.scale && P.out_split.hi) {
-                    esc[cc] = *reinterpret_cast<const float4 *>(P.scale + tn * BLOCK_N + cb + cc * 32 + sub_g * 4);
-                    esh[cc] = *reinterpret_cast<const float4 *>(P.shift + tn * BLOCK_N + cb + cc * 32 + sub_g * 4);
+            for (int h = 0; h < 2; ++h) {
+                const int row = ra + 8 * h;
+                bool valid;
+                int n_img, oy, ox;
+                if (G.flat) {
+                    const long long m = (long long)tm * 128 + row;
+                    valid = m < G.m_total;
+                    const long long hw = (long long)P.ho * P.wo;
+                    n_img = valid ? (int)(m / hw) : 0;
+                    const int r = valid ? (int)(m - (long long)n_img * hw) : 0;
+                    oy = r / P.wo; ox = r - oy * P.wo;
+                } else {
+                    const int per_img = G.tiles_x * G.tiles_y;
+                    n_img = tm / per_img;
+                    const int r = tm - n_img * per_img;
+                    const int ty = r / G.tiles_x, tx = r - ty * G.tiles_x;
+                    const int py = row / G.bw, px = row - py * G.bw;
+                    oy = ty * G.bh + py; ox = tx * G.bw + px;
+                    valid = row < G.bw * G.bh && oy < P.ho && ox < P.wo;
                 }
+                po[h] = pix_offsets<MODE>(P, valid, n_img, oy, ox);
             }
-            float acc[CW];
+            const bool bn = MODE != EPI_UP2 && P.scale && P.out_split.hi;
 #pragma unroll
-            for (int j = 0; j < CW; ++j) acc[j] = 0.f;
-            for (int it0 = 0; it0 < kiters; it0 += G.seg, ++scount) {
-                const int as = scount & 1;
-                const uint32_t aph = (uint32_t)(scount >> 1) & 1u;
-                mbar_wait(tfull_bar(as), aph);
-                tc_fence_after();
-                const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * 2 * BLOCK_N + cb);
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
+                const float2 ws = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
+                float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
+                if (bn) { sc = __ldg(reinterpret_cast<const float2 *>(P.scale + c)); sh = __ldg(reinterpret_cast<const float2 *>(P.shift + c)); }
 #pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += 32) {
-                    uint32_t r[32];
-                    tc_ld32(t_addr + (uint32_t)c0, r);                       // a_hi*w_hi + a_lo*w_hi
-                    tc_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r[j]);
-                    tc_ld32(t_addr + (uint32_t)(BLOCK_N + c0), r);           // a_hi*w_lo
-                    tc_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r[j]);
-                }
-                tc_fence_before();
-                mbar_arrive(tempty_bar(as));  // segment drained: the MMA warp may overwrite this buffer
-            }
-            // Transposed write-out: a thread's accumulator row is one pixel x CW channels; storing it directly
-            // would scatter 8-byte pieces over 32 cache lines per instruction.  Each warp passes 32px x 32ch
-            // blocks through its private (XOR-swizzled) shared-memory tile so that 8 lanes cover the 32
-            // channels of one pixel: 128 B of fp32 / 64 B of fp16 contiguous per pixel per instruction.
-            // Skip loads (upsample mode) of 4 pixels-per-lane are issued before any of them is consumed.
-            const float *res_tile = nullptr;
-            if constexpr (RT) {
-                const int r = tcount_e & 1;
-                mbar_wait(rfull_bar(r), (uint32_t)(tcount_e >> 1) & 1u);
-                res_tile = reinterpret_cast<const float *>(smem_raw + (raw_base + r * RAW_TILE_BYTES - smem_u32(smem_raw)));
-            }
-#pragma unroll
-            for (int c0 = 0; c0 < CW; c0 += 32) {
-#pragma unroll
-                for (int g = 0; g < 8; ++g)
-                    *reinterpret_cast<float4 *>(&ep_tile[lane * 32 + ((g ^ (lane & 7)) << 2)]) =
-                        make_float4(acc[c0 + 4 * g], acc[c0 + 4 * g + 1], acc[c0 + 4 * g + 2], acc[c0 + 4 * g + 3]);
-                __syncwarp();
-                const int ch = tn * BLOCK_N + cb + c0 + sub_g * 4;
-                constexpr int PB = MODE == EPI_UP2 ? (XF ? 2 : 4) : 8;  // pixels-per-lane whose loads are in flight together
-                if (MODE != EPI_UP2 && G.lean_epi) {
-#pragma unroll
-                    for (int it = 0; it < 8; ++it) {
-                        const int src = it * 4 + sub_px;
-                        const long long so = __shfl_sync(0xffffffffu, off_s, src), ro = __shfl_sync(0xffffffffu, off_r, src);
-                        const float4 t = *reinterpret_cast<const float4 *>(&ep_tile[src * 32 + ((sub_g ^ (src & 7)) << 2)]);
-                        const float4 ws = ews[c0 / 32];
-                        float v[4] = {t.x * ws.x, t.y * ws.y, t.z * ws.z, t.w * ws.w};
-                        if constexpr (MODE == EPI_RES) {
-                            float4 r;
-                            if constexpr (RT) r = *reinterpret_cast<const float4 *>(res_tile + (quad * 32 + src) * BLOCK_N + cb + c0 + sub_g * 4);
-                            else r = rpre[c0 / 32][it];
-                            v[0] += r.x; v[1] += r.y; v[2] += r.z; v[3] += r.w;
-                        }
-                        if (ro >= 0) *reinterpret_cast<float4 *>(P.out_raw.p + ro + ch) = make_float4(v[0], v[1], v[2], v[3]);
-                        if (so >= 0) {
-                            if (P.scale) {
-                                const float4 sc = esc[c0 / 32], sh = esh[c0 / 32];
-                                v[0] = v[0] * sc.x + sh.x; v[1] = v[1] * sc.y + sh.y; v[2] = v[2] * sc.z + sh.z; v[3] = v[3] * sc.w + sh.w;
-                            }
-                            if (P.relu) {
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
-                            }
-                            store_split4(P.out_split, so + ch, v);
-                        }
-                    }
-                } else
-#pragma unroll
-                for (int bt = 0; bt < 8 / PB; ++bt) {
-                    int pv[PB], pn[PB], py[PB], px[PB];
-                    EpiPre<MODE> pre[PB];
-#pragma unroll
-                    for (int u = 0; u < PB; ++u) {
-                        const int src = (bt * PB + u) * 4 + sub_px;
-                        pv[u] = __shfl_sync(0xffffffffu, (int)valid, src);
-                        pn[u] = __shfl_sync(0xffffffffu, n_img, src);
-                        py[u] = __shfl_sync(0xffffffffu, oy, src);
-                        px[u] = __shfl_sync(0xffffffffu, ox, src);
-                        if constexpr (RT) pre[u].r = *reinterpret_cast<const float4 *>(res_tile + (quad * 32 + src) * BLOCK_N + cb + c0 + sub_g * 4);
-                        else if constexpr (MODE == EPI_RES) pre[u].r = rpre[c0 / 32][bt * PB + u];
-                        else if (pv[u]) epi_prefetch<MODE>(P, pn[u], py[u], px[u], ch, pre[u]);
-                    }
-#pragma unroll
-                    for (int u = 0; u < PB; ++u) {
-                        const int src = (bt * PB + u) * 4 + sub_px;
-                        const float4 t = *reinterpret_cast<const float4 *>(&ep_tile[src * 32 + ((sub_g ^ (src & 7)) << 2)]);
-                        if (pv[u]) {
-                            float v[4] = {t.x, t.y, t.z, t.w};
-                            epi_finish<MODE>(P, pn[u], py[u], px[u], ch, v, pre[u], esc[c0 / 32], esh[c0 / 32], ews[c0 / 32]);
-                        }
-                    }
-                }
-                __syncwarp();
-            }
-            if constexpr (RT) {  // this warp is done with the residual slot
-                if (lane == 0) mbar_arrive(rempty_bar(tcount_e & 1));
-                ++tcount_e;
+                for (int h = 0; h < 2; ++h)
+                    if (po[h].raw >= 0 || po[h].spl >= 0)
+                        epi_finish2<MODE>(P, po[h], c, sum[4 * j + 2 * h] * ws.x, sum[4 * j + 2 * h + 1] * ws.y, sc, sh);
             }
         }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// AR variant: 1x1 stride-1 convolution + residual with a RESIDENT A operand (the conv3 of the encoder's residual units,
-// reference net_utils.py:233-266; K <= 256, cout = 4K).
-// The RT variant above walks (M-tile, N-tile) pairs and fetches A (128 px x K, hi and lo) and W (64 cout x K) again for
-// each of them: 24 B of L2->SM traffic per output element at K = 256 against the ~11 TB/s the SMs can take while the
-// tensor core runs, i.e. a 190 TFLOP/s cap (measured 167-172).  Here a CTA owns a work unit = one M-tile x `gn`
-// consecutive N-tiles: the A tile is fetched ONCE per unit and stays in shared memory while the unit's W tiles stream
-// through a ring, which leaves 1 (A) + 8 (W) + 4 (residual) B per output element.
-//  * A slices have their own full / empty barriers: the MMA warp releases slice kc right after the unit's LAST tile has
-//    issued its MMAs on it, so the next unit's slice 0 is in flight three slices before the unit ends (no bubble).
-//  * The fp32 residual never meets the epilogue's staging tile: every epilogue warp owns a [32 px][32 ch] fp32 region
-//    (4 KB, 128 B rows, SWIZZLE_128B) that TMA fills with the residual of the warp's own quadrant / column half; the warp
-//    adds its accumulator rows IN PLACE (lane = pixel: conflict-free 16 B accesses thanks to the swizzle), reads the
-//    region back transposed (8 lanes = the 32 channels of one pixel = 128 B coalesced stores) and then requests the
-//    next tile's residual box itself -- no cross-warp hand-off, no separate transpose buffer.
-struct ArGeom {
-    int tiles_m, tiles_n, kchunks, gn, ngroups, wst;
-    int pf;    // L2 prefetch of the next unit's A slices and of residual boxes two tiles ahead (0 = off)
-    int nres;  // residual regions per epilogue warp (1..4, as shared memory allows): that many tiles' residual boxes are in
-               // flight -- the layers this serves sit close to the HBM roofline, bytes in flight are what count
-    long long m_total;
-};
-constexpr int AR_BN = 64;
-constexpr int AR_A_SLICE = 2 * A_TILE_BYTES;          // hi | lo of one 64-channel slice
-constexpr int AR_W_STAGE = 2 * AR_BN * 128;           // [w_hi | w_lo] of one (64-channel, 64-cout) tile
-constexpr int AR_MAX_K = 4, AR_MAX_WST = 8, AR_MAX_NRES = 4;
-
-__global__ void __launch_bounds__(TC_THREADS, 1)
-k_conv_ar(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-          const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
-          const __grid_constant__ CUtensorMap tm_res, const ConvParams P, const ArGeom G) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t w_base = smem_base + (uint32_t)G.kchunks * AR_A_SLICE;
-    const uint32_t r_base = w_base + (uint32_t)G.wst * AR_W_STAGE;       // nres x 8 x 4 KB residual / write-out regions
-    const uint32_t bar_base = r_base + (uint32_t)G.nres * EP_WARPS * 4096u;
-    auto afull_bar = [&](int k) { return bar_base + 8u * k; };
-    auto aempty_bar = [&](int k) { return bar_base + 8u * (AR_MAX_K + k); };
-    auto wfull_bar = [&](int s) { return bar_base + 8u * (2 * AR_MAX_K + s); };
-    auto wempty_bar = [&](int s) { return bar_base + 8u * (2 * AR_MAX_K + AR_MAX_WST + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * AR_MAX_K + 2 * AR_MAX_WST + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * AR_MAX_K + 2 * AR_MAX_WST + 2 + s); };
-    auto rfull_bar = [&](int w, int r) { return bar_base + 8u * (2 * AR_MAX_K + 2 * AR_MAX_WST + 4 + AR_MAX_NRES * w + r); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * AR_MAX_K + 2 * AR_MAX_WST + 4 + AR_MAX_NRES * EP_WARPS);
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr uint32_t TMEM_COLS = 4 * AR_BN;  // two buffers of [hi*hi + lo*hi | hi*lo]
-
-    if (warp == 0 && lane == 0) {
-        for (int k = 0; k < AR_MAX_K; ++k) { mbar_init(afull_bar(k), 1); mbar_init(aempty_bar(k), 1); }
-        for (int s = 0; s < AR_MAX_WST; ++s) { mbar_init(wfull_bar(s), 1); mbar_init(wempty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), EP_WARPS * 32); }
-        for (int w = 0; w < EP_WARPS; ++w)
-            for (int r = 0; r < AR_MAX_NRES; ++r) mbar_init(rfull_bar(w, r), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-    const int units = G.tiles_m * G.ngroups;
-
-    if (warp == 0) {
-        // ===================== TMA producer: A slices once per unit, W tiles per (N-tile, slice) =====================
-        if (lane == 0) {
-            int uc = 0, wit = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x, ++uc) {
-                const int tm = u / G.ngroups, ng = u - tm * G.ngroups;
-                const int m0 = tm * 128;
-                if (G.pf > 0 && u + (int)gridDim.x < units) {  // the next unit's A tile -> L2, a whole unit ahead
-                    const int m0n = ((u + (int)gridDim.x) / G.ngroups) * 128;
-                    if (m0n != m0)
-                        for (int kc = 0; kc < G.kchunks; ++kc) { tma_prefetch_2d(&tm_a_hi, kc * 64, m0n); tma_prefetch_2d(&tm_a_lo, kc * 64, m0n); }
-                }
-                for (int j = 0; j < G.gn; ++j) {
-                    const int tn = ng * G.gn + j;
-                    for (int kc = 0; kc < G.kchunks; ++kc, ++wit) {
-                        if (j == 0) {
-                            mbar_wait(aempty_bar(kc), ((uint32_t)uc & 1u) ^ 1u);
-                            mbar_expect_tx(afull_bar(kc), (uint32_t)AR_A_SLICE);
-                            const uint32_t a = smem_base + (uint32_t)kc * AR_A_SLICE;
-                            tma_2d(a, &tm_a_hi, afull_bar(kc), kc * 64, m0);
-                            tma_2d(a + A_TILE_BYTES, &tm_a_lo, afull_bar(kc), kc * 64, m0);
-                        }
-                        const int s = wit % G.wst;
-                        mbar_wait(wempty_bar(s), (((uint32_t)(wit / G.wst)) & 1u) ^ 1u);
-                        mbar_expect_tx(wfull_bar(s), (uint32_t)AR_W_STAGE);
-                        const uint32_t b = w_base + (uint32_t)s * AR_W_STAGE;
-                        tma_3d(b, &tm_w_hi, wfull_bar(s), kc * 64, tn * AR_BN, 0);
-                        tma_3d(b + AR_BN * 128, &tm_w_lo, wfull_bar(s), kc * 64, tn * AR_BN, 0);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(AR_BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | ((uint32_t)(2 * AR_BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            int uc = 0, wit = 0, tc = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x, ++uc) {
-                for (int j = 0; j < G.gn; ++j, ++tc) {
-                    const int as = tc & 1;
-                    mbar_wait(tempty_bar(as), (((uint32_t)(tc >> 1)) & 1u) ^ 1u);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(as * 2 * AR_BN);
-                    for (int kc = 0; kc < G.kchunks; ++kc, ++wit) {
-                        if (j == 0) mbar_wait(afull_bar(kc), (uint32_t)uc & 1u);
-                        const int s = wit % G.wst;
-                        mbar_wait(wfull_bar(s), ((uint32_t)(wit / G.wst)) & 1u);
-                        tc_fence_after();
-                        const uint32_t sa = smem_base + (uint32_t)kc * AR_A_SLICE;
-                        const uint64_t da_hi = umma_desc(sa), da_lo = umma_desc(sa + A_TILE_BYTES),
-                                       db_hi = umma_desc(w_base + (uint32_t)s * AR_W_STAGE);  // [w_hi | w_lo]: 128 contiguous rows
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t ko = (uint64_t)(2 * k);
-                            tc_mma_f16(d_tmem, da_hi + ko, db_hi + ko, idesc2, (kc > 0 || k > 0) ? 1u : 0u);
-                            tc_mma_f16(d_tmem, da_lo + ko, db_hi + ko, idesc, 1u);
-                        }
-                        tc_commit(wempty_bar(s));
-                        if (j == G.gn - 1) tc_commit(aempty_bar(kc));  // the unit's last use of this A slice
-                    }
-                    tc_commit(tfull_bar(as));
-                }
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 2..9) =====================
-        const int quad = warp & 3, half = (warp - 2) >> 2, widx = warp - 2;
-        const uint32_t reg_addr0 = r_base + (uint32_t)(widx * G.nres) * 4096u;
-        const int sub_px = lane >> 3, sub_g = lane & 7;
-        // lane 0 only: this warp's residual box of the CTA's tl-th tile (units in round-robin order, gn tiles per unit)
-        auto box_of = [&](int tl, int &c0, int &c1) {
-            const int u = blockIdx.x + (tl / G.gn) * (int)gridDim.x;
-            if (u >= units) return false;
-            const int tm = u / G.ngroups;
-            c0 = ((u - tm * G.ngroups) * G.gn + tl % G.gn) * AR_BN + half * 32;
-            c1 = tm * 128 + quad * 32;
-            return true;
-        };
-        auto request_res = [&](int tl) {
-            int c0, c1;
-            if (!box_of(tl, c0, c1)) return;
-            const int r = tl % G.nres;
-            mbar_expect_tx(rfull_bar(widx, r), 4096u);
-            tma_2d(reg_addr0 + (uint32_t)r * 4096u, &tm_res, rfull_bar(widx, r), c0, c1);
-            if (G.pf > 0 && box_of(tl + 2, c0, c1)) tma_prefetch_2d(&tm_res, c0, c1);  // two tiles further on: HBM -> L2
-        };
-        if (lane == 0) for (int r = 0; r < G.nres; ++r) request_res(r);
-        int tc = 0;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            const int tm = u / G.ngroups, ng = u - tm * G.ngroups;
-            const long long mrow0 = (long long)tm * 128 + quad * 32;
-            for (int j = 0; j < G.gn; ++j, ++tc) {
-                const int tn = ng * G.gn + j;
-                const int ch4 = tn * AR_BN + half * 32 + sub_g * 4;   // this lane's 4 channels in the write-out mapping
-                float4 esc = make_float4(1.f, 1.f, 1.f, 1.f), esh = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (P.scale && P.out_split.hi) {
-                    esc = *reinterpret_cast<const float4 *>(P.scale + ch4);
-                    esh = *reinterpret_cast<const float4 *>(P.shift + ch4);
-                }
-                const int as = tc & 1;
-                mbar_wait(tfull_bar(as), ((uint32_t)(tc >> 1)) & 1u);
-                tc_fence_after();
-                const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * 2 * AR_BN + half * 32);
-                uint32_t r0[32], r1[32];
-                tc_ld32(t_addr, r0);                      // a_hi*w_hi + a_lo*w_hi
-                tc_ld32(t_addr + (uint32_t)AR_BN, r1);    // a_hi*w_lo
-                tc_ld_wait();
-                tc_fence_before();
-                mbar_arrive(tempty_bar(as));
-                const int rr = tc % G.nres;
-                uint8_t *reg = smem_raw + (reg_addr0 + (uint32_t)rr * 4096u - smem_u32(smem_raw));
-                mbar_wait(rfull_bar(widx, rr), ((uint32_t)(tc / G.nres)) & 1u);
-                // in place: region[pixel = lane][channel] = acc * 2^-e + residual   (2^-e exact, so fma == mul then add)
-                const float *osc = P.w.oscale + tn * AR_BN + half * 32;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const float4 ws = __ldg(reinterpret_cast<const float4 *>(osc + 4 * c));
-                    float4 *p = reinterpret_cast<float4 *>(reg + lane * 128 + ((c ^ (lane & 7)) << 4));
-                    float4 v = *p;
-                    v.x = fmaf(__uint_as_float(r0[4 * c]) + __uint_as_float(r1[4 * c]), ws.x, v.x);
-                    v.y = fmaf(__uint_as_float(r0[4 * c + 1]) + __uint_as_float(r1[4 * c + 1]), ws.y, v.y);
-                    v.z = fmaf(__uint_as_float(r0[4 * c + 2]) + __uint_as_float(r1[4 * c + 2]), ws.z, v.z);
-                    v.w = fmaf(__uint_as_float(r0[4 * c + 3]) + __uint_as_float(r1[4 * c + 3]), ws.w, v.w);
-                    *p = v;
-                }
-                __syncwarp();
-#pragma unroll
-                for (int it = 0; it < 8; ++it) {
-                    const int px = it * 4 + sub_px;
-                    const float4 t = *reinterpret_cast<const float4 *>(reg + px * 128 + ((sub_g ^ (px & 7)) << 4));
-                    const long long m = mrow0 + px;
-                    if (m < G.m_total) {
-                        if (P.out_raw.p) *reinterpret_cast<float4 *>(P.out_raw.p + m * P.out_raw.sW + ch4) = t;
-                        if (P.out_split.hi) {
-                            float v[4] = {t.x, t.y, t.z, t.w};
-                            if (P.scale) { v[0] = v[0] * esc.x + esh.x; v[1] = v[1] * esc.y + esh.y; v[2] = v[2] * esc.z + esh.z; v[3] = v[3] * esc.w + esh.w; }
-                            if (P.relu) {
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
-                            }
-                            store_split4(P.out_split, m * P.out_split.sW + ch4, v);
-                        }
-                    }
-                }
-                // the region is free: request the next tile's residual (generic accesses above -> async-proxy write below)
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) request_res(tc + G.nres);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// RS variant ("row-stacked"): the decoder's grouped k x k convolutions (128 -> 32 channels in 4 groups, valid padding,
-// reference net_utils.py:101-118: DenseBlock conv2), stored block-diagonal dense.
-// A tcgen05 SS-mode instruction costs max(71.6, N/2) cycles whatever N is (tools/umma_rate_probe.cu): with N = 32 couts
-// the per-tap path issues kh*kw*8*2 = 400 (5x5) instructions of 71.6 cycles per 128 pixels -- 28 TFLOP/s, a tenth of the
-// kernel's time for 1 % of its FLOPs.  Here the kw taps of a filter ROW are stacked along N instead:
-//     D[(y, xi), (kx, c)] = sum_{ky, cin} in[y + ky, xi, cin] * w[ky, kx, cin, c]          N = kw * 32 (160 / 96)
-// for every INPUT column xi of the tile's rows, and the epilogue folds the columns (col2im along x):
-//     out[y, x, c] = sum_kx D[(y, x + kx), (kx, c)].
-// The weight tensor [tap = ky*kw + kx][cout][cin] already IS [ky][(kx, cout)][cin], so a second tensor map over the same
-// memory serves the stacked tiles.  Per K-step: a_hi*w_hi, a_hi*w_lo, a_lo*w_hi as three N = kw*32 instructions into ONE
-// accumulator (3 x 80 cycles at N = 160): 40 K-steps = 9 600 cycles per tile instead of 28 600.
-// M-tile = bh full input rows (bw = input width, bw * bh <= 128); accumulation segments as in k_conv_tc.
-// Epilogue: warps (quad, half) own accumulator rows quad*32.. and channels half*16.. of every kx; they drop their rows
-// into a per-half staging tile (row stride kw*16 + 4 floats: 16-byte accesses by 8 consecutive rows hit 8 different bank
-// groups), meet at a named barrier, and each thread then sums its own pixel's kw shifted rows and stores 64 B of fp32.
-struct RsGeom {
-    int bw, bh, rows, tiles_y, tiles_m, kchunks, kh, seg;
-};
-template <int KW> constexpr int rs_stages() { return KW >= 5 ? 2 : 3; }
-template <int KW> constexpr int rs_max_rows() { return KW >= 5 ? 124 : 128; }   // staging rows that fit beside the operand ring
-template <int KW> constexpr int rs_stage_bytes() { return 2 * A_TILE_BYTES + 2 * KW * 32 * 128; }
-template <int KW> constexpr int rs_smem() {
-    return 1024 + rs_stages<KW>() * rs_stage_bytes<KW>() + 2 * rs_max_rows<KW>() * (KW * 16 + 4) * 4 + 8 * (2 * rs_stages<KW>() + 4) + 16;
-}
-
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-
-template <int KW>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-k_conv_rs(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-          const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
-          const ConvParams P, const RsGeom G) {
-    constexpr int N = KW * 32, STAGES = rs_stages<KW>(), STAGE_BYTES = rs_stage_bytes<KW>();
-    constexpr int W_PLANE = N * 128;                 // one fp16 plane of the stacked weight tile
-    constexpr int NH = KW * 16, STRIDE = NH + 4;     // accumulators per thread; staging row stride in floats
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t st_base = smem_base + STAGES * STAGE_BYTES;                        // 2 halves x [rows][STRIDE] fp32
-    const uint32_t bar_base = st_base + 2u * rs_max_rows<KW>() * STRIDE * 4u;
-    auto full_bar = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr uint32_t TMEM_COLS = 512;              // two accumulation buffers of N <= 160 columns at 0 and 256
-
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), EP_WARPS * 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-    const int kiters = G.kh * G.kchunks;             // K-slices per tile: (filter row, 64-channel slice)
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            const uint32_t tx = (uint32_t)(2 * G.rows * 128 + 2 * W_PLANE);
-            int itg = 0;
-            for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x) {
-                const int n_img = tile / G.tiles_y, y0 = (tile - n_img * G.tiles_y) * G.bh;
-                for (int ky = 0; ky < G.kh; ++ky)
-                    for (int kc = 0; kc < G.kchunks; ++kc, ++itg) {
-                        const int s = itg % STAGES;
-                        mbar_wait(empty_bar(s), (((uint32_t)(itg / STAGES)) & 1u) ^ 1u);
-                        mbar_expect_tx(full_bar(s), tx);
-                        const uint32_t sa = smem_base + (uint32_t)s * STAGE_BYTES;
-                        tma_4d(sa, &tm_a_hi, full_bar(s), kc * 64, 0, y0 + ky, n_img);                 // bh full input rows, shifted by ky
-                        tma_4d(sa + A_TILE_BYTES, &tm_a_lo, full_bar(s), kc * 64, 0, y0 + ky, n_img);
-                        tma_3d(sa + 2 * A_TILE_BYTES, &tm_w_hi, full_bar(s), kc * 64, 0, ky);           // all kx taps of filter row ky
-                        tma_3d(sa + 2 * A_TILE_BYTES + W_PLANE, &tm_w_lo, full_bar(s), kc * 64, 0, ky);
-                    }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            int itg = 0, scount = 0;
-            for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x) {
-                for (int it0 = 0; it0 < kiters; it0 += G.seg, ++scount) {
-                    const int as = scount & 1;
-                    mbar_wait(tempty_bar(as), (((uint32_t)(scount >> 1)) & 1u) ^ 1u);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(as * 256);
-                    const int it1 = min(it0 + G.seg, kiters);
-                    for (int it = it0; it < it1; ++it, ++itg) {
-                        const int s = itg % STAGES;
-                        mbar_wait(full_bar(s), ((uint32_t)(itg / STAGES)) & 1u);
-                        tc_fence_after();
-                        const uint32_t sa = smem_base + (uint32_t)s * STAGE_BYTES;
-                        const uint64_t da_hi = umma_desc(sa), da_lo = umma_desc(sa + A_TILE_BYTES),
-                                       db_hi = umma_desc(sa + 2 * A_TILE_BYTES), db_lo = umma_desc(sa + 2 * A_TILE_BYTES + W_PLANE);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t ko = (uint64_t)(2 * k);
-                            tc_mma_f16(d_tmem, da_hi + ko, db_hi + ko, idesc, (it > it0 || k > 0) ? 1u : 0u);
-                            tc_mma_f16(d_tmem, da_hi + ko, db_lo + ko, idesc, 1u);
-                            tc_mma_f16(d_tmem, da_lo + ko, db_hi + ko, idesc, 1u);
-                        }
-                        tc_commit(empty_bar(s));
-                    }
-                    tc_commit(tfull_bar(as));
-                }
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 2..9): drain segments, fold the kx columns, store =====================
-        const int quad = warp & 3, half = (warp - 2) >> 2;
-        const int row = quad * 32 + lane;               // accumulator row = (input row py, input column px) of the tile
-        float *stage = reinterpret_cast<float *>(smem_raw + (st_base - smem_u32(smem_raw))) + half * rs_max_rows<KW>() * STRIDE;
-        const int py = row / G.bw, px = row - py * G.bw;
-        const float *osc = P.w.oscale + half * 16;
-        int scount = 0;
-        for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x) {
-            const int n_img = tile / G.tiles_y, y0 = (tile - n_img * G.tiles_y) * G.bh;
-            float acc[NH];
-#pragma unroll
-            for (int j = 0; j < NH; ++j) acc[j] = 0.f;
-            for (int it0 = 0; it0 < kiters; it0 += G.seg, ++scount) {
-                const int as = scount & 1;
-                mbar_wait(tfull_bar(as), ((uint32_t)(scount >> 1)) & 1u);
-                tc_fence_after();
-                const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * 256 + half * 16);
-#pragma unroll
-                for (int kx = 0; kx < KW; ++kx) {
-                    uint32_t r[16];
-                    tc_ld16(t_addr + (uint32_t)(kx * 32), r);
-                    tc_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) acc[kx * 16 + j] += __uint_as_float(r[j]);
-                }
-                tc_fence_before();
-                mbar_arrive(tempty_bar(as));
-            }
-            // rows >= G.rows of the MMA tile were never written by TMA (stale shared memory): they stay out of the staging tile
-            if (row < G.rows) {
-                float4 *dst = reinterpret_cast<float4 *>(stage + row * STRIDE);
-#pragma unroll
-                for (int q = 0; q < NH / 4; ++q) dst[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
-            }
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
-            const int oy = y0 + py;
-            if (row < G.rows && px < P.wo && oy < P.ho) {   // px + kx < bw: the kw rows read below belong to the same input row
-                float o[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) o[j] = 0.f;
-#pragma unroll
-                for (int kx = 0; kx < KW; ++kx) {
-                    const float4 *src = reinterpret_cast<const float4 *>(stage + (row + kx) * STRIDE + kx * 16);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const float4 t = src[q];
-                        o[4 * q] += t.x; o[4 * q + 1] += t.y; o[4 * q + 2] += t.z; o[4 * q + 3] += t.w;
-                    }
-                }
-                float *out = P.out_raw.p + n_img * P.out_raw.sN + (long long)oy * P.out_raw.sH + (long long)px * P.out_raw.sW + half * 16;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float4 ws = __ldg(reinterpret_cast<const float4 *>(osc + 4 * q));
-                    *reinterpret_cast<float4 *>(out + 4 * q) = make_float4(o[4 * q] * ws.x, o[4 * q + 1] * ws.y, o[4 * q + 2] * ws.z, o[4 * q + 3] * ws.w);
-                }
-            }
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");   // staging tile free for the next tile
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
     }
 }
 
@@ -1157,13 +485,13 @@ k_conv_rs(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
 // every byte ONCE through a 256-entry table holding (float)v / 255.0f (the reference's own `imgs / 255.0`, an IEEE
 // division) already split into fp16 hi | lo, and keep the converted strip in shared memory; an A row's 16-byte chunk is
 // then 8 consecutive words of that strip (hi halves to one plane, lo halves to the other), written 128B-swizzled where
-// the MMA reads it.  (A first version looked every A element up separately from a byte strip: 49 lookups per input
-// byte, 15 k cycles per tile in shared-memory wavefronts -- 8x the tensor core's time.)  Weights (64 x 192 x {hi, lo} =
-// 48 KB) stay resident in shared memory.
+// wgmma reads it.  Weights (64 x 192 x {hi, lo} = 48 KB) stay resident in shared memory.
 // A tile = 128 consecutive output pixels of one image in raster order (at most two output rows, wo >= 128).
+// Warps: 0 = weight TMA, 4..11 = wgmma consumers (two warpgroups of 64 rows), 12..19 = A-operand producers.
 constexpr int C0T_PROD_WARPS = 8, C0T_STAGES = 3, C0T_K = 192, C0T_ROWS = 8, C0T_STRIDE = 832;
 constexpr int C0T_PSTRIDE = 833;  // words per row of the converted strip: odd, so the 7 filter rows fall into different banks
-constexpr int C0T_THREADS = 64 + EP_WARPS * 32 + C0T_PROD_WARPS * 32;
+constexpr int C0T_PROD0 = 4 + CONS_WARPS;   // first producer warp
+constexpr int C0T_THREADS = (C0T_PROD0 + C0T_PROD_WARPS) * 32;
 constexpr int C0T_SMEM = 1024 + C0T_STAGES * 2 * A_TILE_BYTES + 3 * 2 * 64 * 128 + 2 * C0T_ROWS * C0T_PSTRIDE * 4 + 256 * 4 + 256;
 
 __global__ void __launch_bounds__(C0T_THREADS, 1)
@@ -1181,25 +509,17 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
     const uint32_t bar_base = smem_base + BAR_OFF;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C0T_STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * C0T_STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * C0T_STAGES + 2 + s); };
-    const uint32_t wfull_bar = bar_base + 8u * (2 * C0T_STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C0T_STAGES + 5);
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(smem_gen + BAR_OFF + 8 * (2 * C0T_STAGES + 5));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t wfull_bar = bar_base + 8u * (2 * C0T_STAGES);
+    // warp index broadcast from lane 0: provably warp-uniform, so the role branches below do not count as divergent
+    // paths around the wgmma (ptxas would otherwise serialise them)
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     const int ho = out.h, wo = out.w, hw = ho * wo;
     const int tiles_img = (hw + 127) >> 7, total_tiles = B * tiles_img;
-    constexpr uint32_t TMEM_COLS = 256;  // 2 buffers x [hi*hi + lo*hi | hi*lo] of 64 columns
 
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < C0T_STAGES; ++s) { mbar_init(full_bar(s), C0T_PROD_WARPS); mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), EP_WARPS * 32); }
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < C0T_STAGES; ++s) { mbar_init(full_bar(s), C0T_PROD_WARPS); mbar_init(empty_bar(s), CONS_WARPS); }
         mbar_init(wfull_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     {   // (float)v / 255.0f as fp16 hi | lo
         uint32_t *lut = reinterpret_cast<uint32_t *>(smem_gen + LUT_OFF);
@@ -1209,10 +529,7 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
             lut[i] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     if (warp == 0) {
         if (lane == 0) {  // resident weights: three K-slices, hi and lo
@@ -1222,76 +539,53 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
                 tma_3d(smem_base + W_OFF + s * 16384 + 8192, &tm_w_lo, wfull_bar, s * 64, 0, 0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            mbar_wait(wfull_bar, 0);
-            int it = 0, tc = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tc) {
-                const int as = tc & 1;
-                mbar_wait(tempty_bar(as), ((uint32_t)(tc >> 1) & 1u) ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * 128);
-                for (int ks = 0; ks < 3; ++ks, ++it) {
-                    const int s = it % C0T_STAGES;
-                    mbar_wait(full_bar(s), (uint32_t)(it / C0T_STAGES) & 1u);
-                    tc_fence_after();
-                    const uint32_t sa = smem_base + s * STAGE;
-                    const uint64_t da_hi = umma_desc(sa), da_lo = umma_desc(sa + A_TILE_BYTES),
-                                   db = umma_desc(smem_base + W_OFF + ks * 16384);  // [w_hi | w_lo]: 128 contiguous rows
+    } else if (warp < 4) {
+        // idle warps of the producer warpgroup
+    } else if (warp < C0T_PROD0) {
+        // ===================== wgmma + epilogue: BN+ReLU -> split store =====================
+        const int wg = (warp >> 2) - 1;
+        const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        float acc[32];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t ko = (uint64_t)(2 * k);
-                        tc_mma_f16(d_tmem, da_hi + ko, db + ko, idesc2, (ks > 0 || k > 0) ? 1u : 0u);
-                        tc_mma_f16(d_tmem, da_lo + ko, db + ko, idesc, 1u);
-                    }
-                    tc_commit(empty_bar(s));
-                }
-                tc_commit(tfull_bar(as));
+        for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+        mbar_wait(wfull_bar, 0);
+        int it = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            for (int ks = 0; ks < 3; ++ks, ++it) {
+                const int s = it % C0T_STAGES;
+                mbar_wait(full_bar(s), (uint32_t)(it / C0T_STAGES) & 1u);
+                const uint32_t sa = smem_base + s * STAGE + wg * 64 * 128, sb = smem_base + W_OFF + ks * 16384;
+                wg_fence();
+                mma_slice<64>(acc, sa, sa + A_TILE_BYTES, sb, sb + 8192, ks == 0);
+                wg_commit();
+                wg_wait<0>();
+                wg_fence_regs(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));
             }
-        }
-    } else if (warp < 2 + EP_WARPS) {
-        // ===================== epilogue: TMEM -> BN+ReLU -> split store (64 B of hi and of lo per lane) =====================
-        const int quad = warp & 3, half = (warp - 2) >> 2, cb = half * 32;
-        const int row = quad * 32 + lane;
-        int tc = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tc) {
-            const int n = tile / tiles_img, p = (tile - n * tiles_img) * 128 + row;
-            const int as = tc & 1;
-            mbar_wait(tfull_bar(as), (uint32_t)(tc >> 1) & 1u);
-            tc_fence_after();
-            const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * 128 + cb);
-            uint32_t r0[32], r1[32];
-            tc_ld32(t_addr, r0);
-            tc_ld32(t_addr + 64u, r1);
-            tc_ld_wait();
-            tc_fence_before();
-            mbar_arrive(tempty_bar(as));
-            if (p < hw) {
+            const int n = tile / tiles_img;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int p = (tile - n * tiles_img) * 128 + ra + 8 * h;
+                if (p >= hw) continue;
                 const int oy = p / wo, ox = p - oy * wo;
-                const long long oo = n * out.sN + (long long)oy * out.sH + (long long)ox * out.sW + cb;
+                const long long oo = n * out.sN + (long long)oy * out.sH + (long long)ox * out.sW;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    float t[4];
-                    // per-channel constants straight from the read-only cache (96 registers per thread at 576 threads);
+                    const int c = 8 * j + 2 * (lane & 3);
                     // 2^-e folds into the BN scale exactly
-                    const float4 w4 = __ldg(reinterpret_cast<const float4 *>(oscale + cb + 4 * j));
-                    const float4 s4 = __ldg(reinterpret_cast<const float4 *>(scale + cb + 4 * j));
-                    const float4 b4 = __ldg(reinterpret_cast<const float4 *>(shift + cb + 4 * j));
-                    const float m4[4] = {w4.x * s4.x, w4.y * s4.y, w4.z * s4.z, w4.w * s4.w}, c4[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float v = __uint_as_float(r0[4 * j + i]) + __uint_as_float(r1[4 * j + i]);
-                        t[i] = fmaxf(v * m4[i] + c4[i], 0.f);
-                    }
-                    store_split4(out, oo + 4 * j, t);
+                    const float2 w2 = __ldg(reinterpret_cast<const float2 *>(oscale + c));
+                    const float2 s2 = __ldg(reinterpret_cast<const float2 *>(scale + c));
+                    const float2 b2 = __ldg(reinterpret_cast<const float2 *>(shift + c));
+                    const float t0 = fmaxf(acc[4 * j + 2 * h] * (w2.x * s2.x) + b2.x, 0.f);
+                    const float t1 = fmaxf(acc[4 * j + 2 * h + 1] * (w2.y * s2.y) + b2.y, 0.f);
+                    store_split2(out, oo + c, t0, t1);
                 }
             }
         }
     } else {
-        // ===================== A-operand producers (warps 10..17) =====================
-        const int t = threadIdx.x - (2 + EP_WARPS) * 32;           // 0..255
+        // ===================== A-operand producers (warps 12..19) =====================
+        const int t = threadIdx.x - C0T_PROD0 * 32;                 // 0..255
         const int j = t & 7;                                        // 16-byte chunk of the A row = group inside the K-slice
         const uint32_t *lut = reinterpret_cast<const uint32_t *>(smem_gen + LUT_OFF);
         const int row_bytes = W * 3;
@@ -1365,12 +659,6 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
             asm volatile("bar.sync 2, %0;" ::"n"(C0T_PROD_WARPS * 32) : "memory");  // next strip complete; this one free again
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1393,13 +681,13 @@ static EncodeTiledFn encode_fn() {
 }
 
 static bool encode(unsigned char *dst, void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides_bytes,
-                   const cuuint32_t *box, const cuuint32_t *estr, bool raw_f32 = false, bool swz_f32 = false) {
+                   const cuuint32_t *box, const cuuint32_t *estr, bool raw_f32 = false) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return false;
     alignas(64) CUtensorMap tm;
     CUresult r = fn(&tm, raw_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, base,
                     dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    (raw_f32 && !swz_f32) ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    raw_f32 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return false;
     memcpy(dst, &tm, sizeof(tm));
@@ -1407,34 +695,23 @@ static bool encode(unsigned char *dst, void *base, int rank, const cuuint64_t *d
 }
 
 static int g_force_block_n = 0;
-static int g_seg_chunks = 4;  // 64-channel slices per accumulation segment (4 -> 48 chained MMAs)
-static int g_res_tma = 1, g_res_tma_max_chunks = 4;  // residual tile via TMA for 1x1 layers with K <= 256 (larger K: A re-reads of N=64 tiles cost more)
-// 1x1 + residual layers: A-resident variant (k_conv_ar) instead of RT where K >= g_ar_min_chunks 64-channel slices
-// (0 = never).  Measured on B200 (gpurun_out/r3a_layers_orig16_{base,aronly}.log): d2 (K = 256) 0.194 -> 0.173 ms; d0 / d1
-// (K = 64 / 128) stream 8 B of fp32 residual per output element for 2K FLOPs and sit at the HBM roofline either way.
-// Region sets: 2 beat 1 on K <= 128; 3-4 sets are SLOWER (they shorten the weight ring to 4 stages: d0 0.484 -> 0.531 ms,
-// d1 0.270 -> 0.287), and a 2-stage weight ring costs d2 19 % (gpurun_out/r3f_ab_*.log).
-static int g_ar = 1, g_ar_min_chunks = 1, g_ar_nres = 2, g_ar_min_wst = 3;
-void tc_set_ar_min_wst(int n) { g_ar_min_wst = n < 2 ? 2 : n; }
-void tc_set_ar(int on) { g_ar = on; }
-void tc_set_ar_min_chunks(int n) { g_ar_min_chunks = n; }
-void tc_set_ar_nres(int n) { g_ar_nres = n; }
-static int g_pf = 4;        // L2 prefetch distance (K-slices) for flat operands; 0 = off
-void tc_set_prefetch(int n) { g_pf = n < 0 ? 0 : n; }
-static int g_rs = 1;   // grouped k x k decoder layers: row-stacked kernel (k_conv_rs) instead of the per-tap / HALO path
-void tc_set_rowstack(int on) { g_rs = on; }
-static int g_lean_epi = 1;
-void tc_set_lean_epi(int on) { g_lean_epi = on; }
-static int g_xf_early = 1;
-void tc_set_xf_early(int on) { g_xf_early = on; }
+static int g_seg_chunks = 4;  // 64-channel slices per accumulation segment (4 -> 48 chained wgmma)
+static int g_pf = 4;          // L2 prefetch distance (K-slices) for flat operands; 0 = off
 static int g_xf_trunc = 1;
+void tc_set_prefetch(int n) { g_pf = n < 0 ? 0 : n; }
 void tc_set_xf_trunc(int on) { g_xf_trunc = on; }
-static int g_halo = 1;  // 0 off, 1 auto (where the fixed 8 x 16 tiling fits the output map), 2 every eligible layer
-void tc_set_halo(int mode) { g_halo = mode; }
-void tc_set_res_tma(int on) { g_res_tma = on; }
-void tc_set_res_tma_max_chunks(int n) { g_res_tma_max_chunks = n; }
 void tc_set_block_n(int n) { g_force_block_n = n; }
 void tc_set_seg_chunks(int n) { g_seg_chunks = n < 1 ? 1 : n; }
+
+static int num_sms() {
+    static int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    }
+    return sms;
+}
 
 bool tc_plan(const ConvParams &P, TcPlan &plan) {
     plan.ok = false;
@@ -1452,7 +729,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
     if (xf) {
         if (w.taps != 1 || P.stride != 1 || P.pad_t != 0 || P.res.p) return false;
         if ((reinterpret_cast<uintptr_t>(P.a_raw.p) & 15) || (P.a_raw.sW % 4) || (P.a_raw.sH % 4) || (P.a_raw.sN % 4)) return false;
-        if ((long long)P.B * P.a_raw.sN >= (1ll << 31)) return false;  // 32-bit element offsets in the transform warps
+        if ((long long)P.B * P.a_raw.sN >= (1ll << 31)) return false;
     } else {
         if ((reinterpret_cast<uintptr_t>(P.a.hi) & 15) || (reinterpret_cast<uintptr_t>(P.a.lo) & 15)) return false;
         if ((P.a.sW % 8) || (P.a.sH % 8) || (P.a.sN % 8)) return false;
@@ -1471,91 +748,6 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
     }
     if (xf && bn != 128 && bn != 64) return false;
     cuuint32_t ones[4] = {1, 1, 1, 1};
-    plan.res_tma = 0; plan.ar = 0; plan.ar_gn = 1;
-    if (P.res.p && !P.up2 && !two && !xf && plan.flat && g_res_tma && w.cout % 64 == 0 && w.cin_pad / 64 <= g_res_tma_max_chunks) {
-        const RawRef &r = P.res;
-        const bool dense_r = (long long)r.sW * r.w == r.sH && (long long)r.sH * r.h == r.sN && r.h == P.ho && r.w == P.wo;
-        if (dense_r && !(reinterpret_cast<uintptr_t>(r.p) & 15) && r.sW % 4 == 0) {
-            cuuint64_t rdims[2] = {(cuuint64_t)w.cout, (cuuint64_t)((long long)P.B * r.h * r.w)};
-            cuuint64_t rstr[1] = {(cuuint64_t)r.sW * 4};
-            cuuint32_t rbox[2] = {64, 128};
-            if (encode(plan.tmap_a2_hi, r.p, 2, rdims, rstr, rbox, ones, true)) { plan.res_tma = 1; bn = 64; plan.block_n = 64; }
-            // AR (resident A operand): flat pixel-major addressing of the outputs, residual boxes of [32 px][32 ch] fp32
-            // with the 128 B swizzle (tmap_a2_lo, free in this mode)
-            auto dense_out = [&](long long sW, long long sH, long long sN, int h, int wd) {
-                return sW * wd == sH && sH * h == sN && h == P.ho && wd == P.wo && sW % 4 == 0;
-            };
-            const bool raw_ok = !P.out_raw.p || (dense_out(P.out_raw.sW, P.out_raw.sH, P.out_raw.sN, P.out_raw.h, P.out_raw.w) &&
-                                                 !(reinterpret_cast<uintptr_t>(P.out_raw.p) & 15));
-            const bool split_ok = !P.out_split.hi || (dense_out(P.out_split.sW, P.out_split.sH, P.out_split.sN, P.out_split.h, P.out_split.w) &&
-                                                      !(reinterpret_cast<uintptr_t>(P.out_split.hi) & 7) && !(reinterpret_cast<uintptr_t>(P.out_split.lo) & 7));
-            cuuint32_t abox[2] = {32, 32};
-            if (plan.res_tma && raw_ok && split_ok && w.cin_pad / 64 <= AR_MAX_K && (long long)P.B * r.h * r.w < (1ll << 31) - 256 &&
-                encode(plan.tmap_a2_lo, r.p, 2, rdims, rstr, abox, ones, true, true)) {
-                // work units = M-tiles x groups of gn N-tiles; gn = the divisor of tiles_n with the smallest estimated
-                // time on the SMs: waves x (gn tiles + the exposed part of the A fetch)
-                int sms = 148;
-                { int dev = 0; if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-                const int kch = w.cin_pad / 64, tn = w.cout / 64;
-                const long long tmn = cdiv((long long)P.B * P.ho * P.wo, 128);
-                const double t_tile = std::max(kch * 572.0, (kch * 16384.0 + 32768.0) / 45.0), t_a = kch * 32768.0 / 45.0 * 0.5;
-                double best = 1e30; int best_gn = 1;
-                for (int gn = 1; gn <= tn; ++gn) {
-                    if (tn % gn) continue;
-                    const long long units = tmn * (tn / gn);
-                    const double t = (double)cdiv(units, sms) * (gn * t_tile + t_a);
-                    if (t < best * 0.999) { best = t; best_gn = gn; }
-                    else if (t <= best * 1.001) best_gn = gn;   // ties: the larger group re-reads A less often
-                }
-                plan.ar = 1; plan.ar_gn = best_gn;
-            }
-        }
-    }
-    // RS (row-stacked) variant for the decoder's grouped k x k layers: second A map (full input rows) in tmap_a2_hi / lo,
-    // stacked weight maps over the same [tap][cout][cin] memory read as [ky][(kx, cout)][cin]
-    plan.rs = 0;
-    if (w.taps > 1 && w.kh == w.kw && (w.kw == 3 || w.kw == 5) && P.stride == 1 && P.pad_t == 0 && w.cout == 32 && w.cin_pad == 128 &&
-        !xf && !two && !P.up2 && !P.res.p && P.out_raw.p && !P.out_split.hi && P.a.w == P.wo + w.kw - 1 && P.a.h == P.ho + w.kh - 1 &&
-        !(reinterpret_cast<uintptr_t>(P.out_raw.p) & 15) && P.out_raw.sW % 4 == 0 && P.out_raw.sH % 4 == 0 && P.out_raw.sN % 4 == 0) {
-        const int max_rows = w.kw == 5 ? rs_max_rows<5>() : rs_max_rows<3>();
-        if (P.a.w <= max_rows) {
-            const int bw = P.a.w, bh = std::max(1, std::min(max_rows / bw, P.ho));
-            cuuint64_t dims[4] = {(cuuint64_t)P.a.c, (cuuint64_t)P.a.w, (cuuint64_t)P.a.h, (cuuint64_t)P.B};
-            cuuint64_t str[3] = {(cuuint64_t)P.a.sW * 2, (cuuint64_t)P.a.sH * 2, (cuuint64_t)P.a.sN * 2};
-            cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-            cuuint64_t wdims[3] = {(cuuint64_t)w.cin_pad, (cuuint64_t)(w.kw * w.cout), (cuuint64_t)w.kh};
-            cuuint64_t wstr[2] = {(cuuint64_t)w.cin_pad * 2, (cuuint64_t)w.cin_pad * w.cout * w.kw * 2};
-            cuuint32_t wbox[3] = {64, (cuuint32_t)(w.kw * w.cout), 1};
-            if (encode(plan.tmap_a2_hi, P.a.hi, 4, dims, str, box, ones) && encode(plan.tmap_a2_lo, P.a.lo, 4, dims, str, box, ones) &&
-                encode(plan.tmap_rs_w_hi, w.hi, 3, wdims, wstr, wbox, ones) && encode(plan.tmap_rs_w_lo, w.lo, 3, wdims, wstr, wbox, ones)) {
-                plan.rs = 1; plan.rs_bw = bw; plan.rs_bh = bh;
-            }
-        }
-    }
-    plan.halo = 0;
-    bool want_halo = g_halo && w.taps > 1 && P.stride == 1 && !xf && !two && !P.up2 && !P.res.p && w.kh <= 5 && w.kw <= 5;
-    if (want_halo && g_halo == 1) {
-        // auto: the halo variant tiles the output in fixed 8 x 16 rectangles; take it only where that wastes at most
-        // ~7 % more accumulator rows than the best free-form rectangle of the per-tap path (measured per layer:
-        // 1.05-1.10x where the tilings match, a loss on the small odd-sized decoder maps)
-        double best = 0;
-        for (int bw = 1; bw <= 128; ++bw)
-            for (int bh = std::min(128 / bw, 256); bh >= 1; --bh)
-                best = std::max(best, (double)P.ho * P.wo / ((double)cdiv(P.wo, bw) * cdiv(P.ho, bh) * 128.0));
-        const double cov = (double)P.ho * P.wo / ((double)cdiv(P.wo, 8) * cdiv(P.ho, 16) * 128.0);
-        want_halo = cov >= 0.93 * best;
-    }
-    if (want_halo) {
-        plan.halo = 1;
-        plan.bw = 8; plan.bh = 16;   // one 8-pixel row per swizzle group, 16 rows = the 128 accumulator rows
-        plan.halo_w = plan.bw + w.kw - 1; plan.halo_h = plan.bh + w.kh - 1;
-        plan.tiles_x = cdiv(P.wo, plan.bw); plan.tiles_y = cdiv(P.ho, plan.bh);
-        cuuint64_t dims[4] = {(cuuint64_t)P.a.c, (cuuint64_t)P.a.w, (cuuint64_t)P.a.h, (cuuint64_t)P.B};
-        cuuint64_t str[3] = {(cuuint64_t)P.a.sW * 2, (cuuint64_t)P.a.sH * 2, (cuuint64_t)P.a.sN * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)plan.halo_w, (cuuint32_t)plan.halo_h, 1};
-        if (!encode(plan.tmap_a_hi, P.a.hi, 4, dims, str, box, ones)) return false;
-        if (!encode(plan.tmap_a_lo, P.a.lo, 4, dims, str, box, ones)) return false;
-    } else
     if (plan.flat) {
         cuuint64_t dims[2] = {(cuuint64_t)P.a.c, (cuuint64_t)((long long)P.B * P.a.h * P.a.w)};
         cuuint64_t str[1] = {(cuuint64_t)P.a.sW * 2};
@@ -1624,82 +816,36 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
     return true;
 }
 
-template <int BLOCK_N, int STAGES, int MODE, bool XF, bool RT = false>
+template <int BLOCK_N, int STAGES, int MODE, bool XF>
 static void launch_tm(const ConvParams &P, const TcPlan &plan, const TcGeom &G, cudaStream_t s) {
-    constexpr int smem = STAGES * tc_stage_bytes<BLOCK_N>() + 8 * (2 * STAGES + 4) + 48 + EP_WARPS * 32 * 32 * 4 + 1024 +
-                         ((XF || RT) ? 1024 + 2 * 128 * 64 * 4 : 0);
-    static_assert(smem <= 232448, "shared memory budget exceeded");
+    constexpr int smem = tc_smem<BLOCK_N, STAGES, XF>();
+    static_assert(smem <= SMEM_LIMIT, "shared memory budget exceeded");
     static bool attr = false;
     if (!attr) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, MODE, XF, RT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, MODE, XF>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr = true;
     }
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    int grid = std::min(G.tiles_m * G.tiles_n, sms);
+    const int grid = std::min(G.tiles_m * G.tiles_n, num_sms());
     CUtensorMap a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo;
     memcpy(&a_hi, plan.tmap_a_hi, 128); memcpy(&a_lo, plan.tmap_a_lo, 128);
     memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
     memcpy(&a2_hi, plan.tmap_a2_hi, 128); memcpy(&a2_lo, plan.tmap_a2_lo, 128);
-    k_conv_tc<BLOCK_N, STAGES, MODE, XF, RT><<<grid, TC_THREADS + (XF ? xf_warps<BLOCK_N>() * 32 : 0), smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
+    k_conv_tc<BLOCK_N, STAGES, MODE, XF><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
 }
 
-template <int BLOCK_N, int STAGES> constexpr int halo_fixed_smem() {
-    return STAGES * 2 * BLOCK_N * 128 + 8 * (2 * STAGES + 4) + 48 + EP_WARPS * 32 * 32 * 4 + 1024 + 1024;
-}
-
-// HALO variant: weight ring of STAGES tiles + `na` halo slots (two fp16 planes each) behind the epilogue tiles.
-template <int BLOCK_N, int STAGES>
-static bool launch_halo(const ConvParams &P, const TcPlan &plan, TcGeom G, cudaStream_t s, int min_na) {
-    constexpr int fixed = halo_fixed_smem<BLOCK_N, STAGES>();
-    const int slot = 2 * G.a_plane;
-    G.na = fixed + 2 * slot <= SMEM_LIMIT ? 2 : (fixed + slot <= SMEM_LIMIT ? 1 : 0);
-    if (G.na < min_na) return false;
-    const int smem = fixed + G.na * slot;
-    static int attr_smem = 0;
-    if (smem > attr_smem) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, EPI_PLAIN, false, false, true>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr_smem = smem;
-    }
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    int grid = std::min(G.tiles_m * G.tiles_n, sms);
-    CUtensorMap a_hi, a_lo, w_hi, w_lo;
-    memcpy(&a_hi, plan.tmap_a_hi, 128); memcpy(&a_lo, plan.tmap_a_lo, 128);
-    memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
-    k_conv_tc<BLOCK_N, STAGES, EPI_PLAIN, false, false, true><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a_hi, a_lo, P, G);
-    return true;
-}
-
-template <int BLOCK_N, int STAGES>
+// STAGES: as many operand slots as fit 227 KB beside the XF staging ring (BLOCK_N = 128: 64 KB a slot).
+template <int BLOCK_N, int STAGES, int XSTAGES>
 static void launch_t(const ConvParams &P, const TcPlan &plan, const TcGeom &G, cudaStream_t s) {
     if (P.in_scale) {  // transformed input: only the shapes the plan produces (1x1, plain or upsample epilogue)
         if constexpr (BLOCK_N == 128 || BLOCK_N == 64) {
-            // 2 operand stages: shared memory also holds the raw staging ring.  An in-place
-            // variant (raw tile landing in the stage's A region, 3 / 4 stages, no ring) was measured SLOWER on B200
-            // (d2 conv1 251 -> 207 TFLOP/s, gpurun_out/r2b_layers_orig16.log): all loads of a slice had to complete and
-            // meet at a barrier before the first store, which cost more than the extra stage of TMA look-ahead gave.
-            constexpr int XS = 2;
-            if (P.up2) launch_tm<BLOCK_N, XS, EPI_UP2, true>(P, plan, G, s);
-            else launch_tm<BLOCK_N, XS, EPI_PLAIN, true>(P, plan, G, s);
+            if (P.up2) launch_tm<BLOCK_N, XSTAGES, EPI_UP2, true>(P, plan, G, s);
+            else launch_tm<BLOCK_N, XSTAGES, EPI_PLAIN, true>(P, plan, G, s);
             return;
         }
         throw Error(-1, "conv_tc: transformed input with unsupported tile shape");
     }
     if (P.up2) launch_tm<BLOCK_N, STAGES, EPI_UP2, false>(P, plan, G, s);
-    else if (P.res.p) {
-        if constexpr (BLOCK_N == 64) { if (plan.res_tma) { launch_tm<64, 2, EPI_RES, false, true>(P, plan, G, s); return; } }
-        launch_tm<BLOCK_N, STAGES, EPI_RES, false>(P, plan, G, s);
-    }
+    else if (P.res.p) launch_tm<BLOCK_N, STAGES, EPI_RES, false>(P, plan, G, s);
     else launch_tm<BLOCK_N, STAGES, EPI_PLAIN, false>(P, plan, G, s);
 }
 
@@ -1713,16 +859,11 @@ bool conv0_tc_supported(int H, int W, int pad, const SplitRef &out) {
 void launch_conv0_tc(const uint8_t *img, int B, int H, int W, int pad, const ConvWeights &w, const float *scale,
                      const float *shift, const SplitRef &out, cudaStream_t s) {
     HVN_CHECK(w.taps == 1 && w.cout == 64 && w.cin_pad == C0T_K, -1, "conv0_tc: unexpected weight layout");
+    static_assert(C0T_SMEM <= SMEM_LIMIT, "conv0_tc: shared memory budget exceeded");
     static bool attr = false;
     if (!attr) {
         HVN_CUDA(cudaFuncSetAttribute(k_conv0_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, C0T_SMEM));
         attr = true;
-    }
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     }
     alignas(64) CUtensorMap w_hi, w_lo;
     cuuint32_t ones[3] = {1, 1, 1};
@@ -1732,76 +873,10 @@ void launch_conv0_tc(const uint8_t *img, int B, int H, int W, int pad, const Con
     HVN_CHECK(encode((unsigned char *)&w_hi, w.hi, 3, dims, str, box, ones) && encode((unsigned char *)&w_lo, w.lo, 3, dims, str, box, ones),
               -2, "conv0_tc: tensor map encode failed");
     const int tiles = B * cdiv((long long)out.h * out.w, 128);
-    k_conv0_tc<<<std::min(tiles, sms), C0T_THREADS, C0T_SMEM, s>>>(w_hi, w_lo, img, B, H, W, pad, w.oscale, scale, shift, out);
-}
-
-static void launch_ar(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
-    ArGeom G;
-    G.kchunks = P.w.cin_pad / 64;
-    G.m_total = (long long)P.B * P.ho * P.wo;
-    G.tiles_m = cdiv(G.m_total, 128);
-    G.tiles_n = P.w.cout / AR_BN;
-    G.gn = plan.ar_gn; G.ngroups = G.tiles_n / G.gn;
-    G.pf = g_pf;
-    int fixed = 1024 + G.kchunks * AR_A_SLICE + EP_WARPS * 4096 + 8 * (2 * AR_MAX_K + 2 * AR_MAX_WST + 4 + AR_MAX_NRES * EP_WARPS) + 16;
-    // residual region sets: as many as fit beside a weight ring of g_ar_min_wst stages (bytes in flight on the fp32 residual
-    // stream are what these HBM-bound layers need), at most g_ar_nres
-    G.nres = 1;
-    while (G.nres < std::min(g_ar_nres, AR_MAX_NRES) && fixed + G.nres * EP_WARPS * 4096 + g_ar_min_wst * AR_W_STAGE <= SMEM_LIMIT) ++G.nres;
-    fixed += (G.nres - 1) * EP_WARPS * 4096;
-    G.wst = std::min(AR_MAX_WST, (SMEM_LIMIT - fixed) / AR_W_STAGE);
-    HVN_CHECK(G.wst >= 2, -1, "conv_ar: weight ring does not fit shared memory");
-    const int smem = fixed + G.wst * AR_W_STAGE;
-    static int attr_smem = 0;
-    if (smem > attr_smem) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv_ar, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr_smem = smem;
-    }
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    const int grid = std::min(G.tiles_m * G.ngroups, sms);
-    CUtensorMap a_hi, a_lo, w_hi, w_lo, res;
-    memcpy(&a_hi, plan.tmap_a_hi, 128); memcpy(&a_lo, plan.tmap_a_lo, 128);
-    memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
-    memcpy(&res, plan.tmap_a2_lo, 128);
-    k_conv_ar<<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, res, P, G);
-}
-
-template <int KW>
-static void launch_rs(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
-    RsGeom G;
-    G.bw = plan.rs_bw; G.bh = plan.rs_bh; G.rows = G.bw * G.bh;
-    G.tiles_y = cdiv(P.ho, G.bh); G.tiles_m = P.B * G.tiles_y;
-    G.kchunks = P.w.cin_pad / 64; G.kh = P.w.kh; G.seg = g_seg_chunks;
-    constexpr int smem = rs_smem<KW>();
-    static_assert(smem <= SMEM_LIMIT, "conv_rs: shared memory budget exceeded");
-    static bool attr = false;
-    if (!attr) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv_rs<KW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr = true;
-    }
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    CUtensorMap a_hi, a_lo, w_hi, w_lo;
-    memcpy(&a_hi, plan.tmap_a2_hi, 128); memcpy(&a_lo, plan.tmap_a2_lo, 128);
-    memcpy(&w_hi, plan.tmap_rs_w_hi, 128); memcpy(&w_lo, plan.tmap_rs_w_lo, 128);
-    k_conv_rs<KW><<<std::min(G.tiles_m, sms), TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, P, G);
+    k_conv0_tc<<<std::min(tiles, num_sms()), C0T_THREADS, C0T_SMEM, s>>>(w_hi, w_lo, img, B, H, W, pad, w.oscale, scale, shift, out);
 }
 
 void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
-    if (plan.rs && g_rs) {
-        if (P.w.kw == 5) launch_rs<5>(P, plan, s); else launch_rs<3>(P, plan, s);
-        return;
-    }
-    if (plan.ar && g_ar && P.w.cin_pad / 64 >= g_ar_min_chunks) { launch_ar(P, plan, s); return; }  // else: the RT variant
     TcGeom G;
     G.flat = plan.flat; G.bw = plan.bw; G.bh = plan.bh; G.tiles_x = plan.tiles_x; G.tiles_y = plan.tiles_y;
     G.kchunks = P.w.cin_pad / 64;
@@ -1810,26 +885,12 @@ void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
     G.m_total = (long long)P.B * P.ho * P.wo;
     G.tiles_m = plan.flat ? cdiv(G.m_total, 128) : P.B * plan.tiles_x * plan.tiles_y;
     G.tiles_n = P.w.cout / plan.block_n;
-    G.halo_w = plan.halo_w; G.halo_h = plan.halo_h; G.na = 0;
     G.xf_trunc = g_xf_trunc;
-    G.xf_early = g_xf_early;
-    G.lean_epi = g_lean_epi;
     G.pf = g_pf;
-    G.a_plane = (plan.halo_w * plan.halo_h * 128 + 1023) & ~1023;
-    if (plan.halo) {
-        bool ok = false;
-        switch (plan.block_n) {
-        case 128: ok = launch_halo<128, 3>(P, plan, G, s, 1); break;
-        case 64: ok = launch_halo<64, 6>(P, plan, G, s, 2) || launch_halo<64, 4>(P, plan, G, s, 1); break;
-        default: ok = launch_halo<32, 8>(P, plan, G, s, 1); break;
-        }
-        if (!ok) throw Error(-1, "conv_tc: halo tile does not fit shared memory");
-        return;
-    }
     switch (plan.block_n) {
-    case 128: launch_t<128, 3>(P, plan, G, s); break;
-    case 64: launch_t<64, 4>(P, plan, G, s); break;
-    default: launch_t<32, 4>(P, plan, G, s); break;
+    case 128: launch_t<128, 3, 2>(P, plan, G, s); break;
+    case 64: launch_t<64, 4, 3>(P, plan, G, s); break;
+    default: launch_t<32, 5, 2>(P, plan, G, s); break;
     }
 }
 

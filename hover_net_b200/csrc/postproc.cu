@@ -1,4 +1,4 @@
-// Instance post-processing on the device (sm_100a): the GPU side of reference
+// Instance post-processing on the device (sm_90a): the GPU side of reference
 // `process` / `__proc_np_hv` (models/hovernet/post_proc.py:26-90, 94-186).
 //
 // Bit-exact contract (tests/test_postproc_gpu.py): every integer result (foreground mask, markers,

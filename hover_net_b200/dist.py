@@ -1,6 +1,6 @@
 """Multi-GPU plumbing: tiles shard by index across ranks (one process per GPU, weights replicated
 once), and the only exchange is the end-of-batch gather of the variable-length instance tables to
-every rank -- the B200 replacement for the reference's single-process `torch.nn.DataParallel`
+every rank -- the multi-GPU replacement for the reference's single-process `torch.nn.DataParallel`
 scatter/gather (reference infer/base.py:69, run_infer.py:139).  Works on any torch.distributed
 backend (NCCL on the GPUs; gloo in the CPU tests)."""
 try:  # torch is only needed for the multi-rank paths; single-GPU tile / WSI runs work without it

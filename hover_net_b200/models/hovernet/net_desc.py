@@ -1,7 +1,7 @@
 """Drop-in for reference `models/hovernet/net_desc.py`: `create_model` (net_desc.py:149) returns an
 object the reference's loader can treat like the torch module it replaces --
 `load_state_dict(strict=True)`, `.to()`, `.eval()` -- while the network itself lives in libhvn
-(hand-written sm_100a kernels).  `torch.nn.DataParallel(net)` is unnecessary: one process per GPU."""
+(hand-written sm_90a kernels).  `torch.nn.DataParallel(net)` is unnecessary: one process per GPU."""
 import numpy as np
 
 from ... import _lib

@@ -14,7 +14,7 @@ import argparse
 import logging
 import os
 
-VERSION = "HoVer-Net B200 Inference v1.0"
+VERSION = "HoVer-Net H100 Inference v1.0"
 
 
 def _top_parser():

@@ -1,4 +1,4 @@
-/* libhvn -- C ABI of the B200-native HoVer-Net tile-inference + instance post-processing engine.
+/* libhvn -- C ABI of the H100-native HoVer-Net tile-inference + instance post-processing engine.
  *
  * Drop-in boundary for the reference's plugin seam (reference infer/base.py:56-78): the three
  * callables the reference resolves by name map onto these entry points
@@ -68,21 +68,16 @@ int hvn_param_info(const hvn_ctx *ctx, int index, const char **name, int *ndim, 
 int hvn_load_param(hvn_ctx *ctx, const char *name, const float *data, int ndim, const int64_t *shape);
 int hvn_finalize_weights(hvn_ctx *ctx);
 
-/* ---- options.  keys: "conv_path" = 0 auto (tcgen05 where eligible), 1 CUDA-core referee only,
- *                      2 = auto + run every tcgen05 layer against the referee kernel and record the
+/* ---- options.  keys: "conv_path" = 0 auto (wgmma where eligible), 1 CUDA-core referee only,
+ *                      2 = auto + run every wgmma layer against the referee kernel and record the
  *                      per-layer max differences (hvn_debug_log);
  *                      "chunk" = patches per internal sub-batch (0 = auto);
  *                      "act_shift" = s in 0..48: store activations as x * 2^-s (see HVN_ERR_RANGE; weights are
  *                      re-derived, results are unchanged because powers of two are exact);
  *                      "profile" = 0 | 1 | 2 (see hvn_stage_ms);
- *                      tuning knobs (defaults are the measured best): "tc_halo" = 0 | 1 | 2 (k x k layers read
- *                      shifted windows of one halo tile: off / where its 8x16 tiling fits / every eligible layer),
- *                      "tc_seg_chunks" (64-channel slices per accumulation segment), "tc_block_n", "tc_res_tma",
- *                      "tc_rowstack" = 0 | 1 (grouped k x k layers on the row-stacked kernel k_conv_rs),
- *                      "tc_ar" = 0 | 1, "tc_ar_min_chunks", "tc_ar_nres", "tc_ar_min_wst" (1x1 + residual layers on the
- *                      A-resident kernel k_conv_ar: smallest K in 64-channel slices, residual region sets per warp, minimum
- *                      weight-ring depth), "tc_prefetch" (L2 prefetch distance in K-slices for flat operands, 0 = off),
- *                      "tc_xf_trunc", "tc_xf_early", "tc_lean_epi" (XF producer / write-out variants; 0 = the older path),
+ *                      tuning knobs: "tc_seg_chunks" (64-channel slices per accumulation segment), "tc_block_n",
+ *                      "tc_prefetch" (L2 prefetch distance in K-slices for flat operands, 0 = off), "tc_xf_trunc"
+ *                      (XF transform: truncating hi/lo split 1, round-to-nearest 0),
  *                      "xform", "fuse_shortcut", "fuse_up2", "branch_streams", "flood_impl".
  *                      The tc_* knobs are process-wide launch-time switches; every setting gives the same results to
  *                      fp32-accumulation noise (tests/test_cnn_gpu.py::test_kernel_variants_agree). */

@@ -233,14 +233,14 @@ def test_tensor_core_stem_equals_cuda_core_stem():
 
 @pytest.mark.parametrize("mode,nt", [("original", 5), ("fast", 6)])
 def test_kernel_variants_agree(mode, nt):
-    """The round-2 kernel variants against the paths they replace, end to end on the same patches: k_conv_rs (row-stacked
-    grouped k x k) vs per-tap / HALO, k_conv_ar (A-resident conv3 + residual) vs RT, and the XF producer options
-    (truncating split, early raw-slot release, L2 prefetch).  Same network output to fp32-accumulation noise."""
+    """The kernel variants against the paths they replace, end to end on the same patches: the XF transform's truncating
+    split vs round-to-nearest, the L2 prefetch cursor on and off, and the fused pre-activation transform (xform) vs a
+    separate BN+ReLU pass.  Same network output to fp32-accumulation noise."""
     from hover_net_b200.models.hovernet.run_desc import infer_step
     net = _model(mode, nt, 0)
     x = synth.make_patches(2, arch.PATCH_GEOMETRY[mode][0], seed=23)
-    knobs = ("tc_rowstack", "tc_ar", "tc_xf_trunc", "tc_xf_early", "tc_prefetch")
-    default = {"tc_rowstack": 1, "tc_ar": 1, "tc_xf_trunc": 1, "tc_xf_early": 1, "tc_prefetch": 4}
+    knobs = ("tc_xf_trunc", "tc_prefetch", "xform")
+    default = {"tc_xf_trunc": 1, "tc_prefetch": 4, "xform": 1}
     try:
         ref = infer_step(x, net)
         assert np.isfinite(ref).all()

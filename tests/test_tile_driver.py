@@ -199,7 +199,7 @@ def test_config3_tile_sharded_over_two_gpus_equals_single_gpu():
     all_reduce (disjoint supports) == the single-GPU device path, bit for bit, on both ranks."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import socket
     import torch.multiprocessing as mp
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()

@@ -50,15 +50,13 @@ if __name__ == "__main__":
 
 
 def _knobs(net):
-    """development knobs from the environment: HVN_TC_HALO=0|1|2"""
-    if os.environ.get("HVN_TC_HALO"):
-        net.ctx.set_option("tc_halo", int(os.environ["HVN_TC_HALO"]))
+    """development knobs from the environment: HVN_TC_SEG=<64-channel slices per accumulation segment>"""
     if os.environ.get("HVN_TC_SEG"):
         net.ctx.set_option("tc_seg_chunks", int(os.environ["HVN_TC_SEG"]))
 
 
 def tc(mode="fast", nt=6, verbose=False):
-    """per-layer tcgen05-vs-referee self test (conv_path=2), then the end-to-end check"""
+    """per-layer wgmma-vs-referee self test (conv_path=2), then the end-to-end check"""
     import re
     from hover_net_b200.models.hovernet.net_desc import create_model
     nt = {"fast": 6, "original": 5}[mode]
@@ -209,7 +207,7 @@ def ab(mode="original", B=16, configs=("base:",), reps=5):
         tag, _, opts = c.partition(":")
         cfgs.append((tag, [(kv.split("=")[0], int(kv.split("=")[1])) for kv in opts.split(",") if "=" in kv]))
     keys = sorted({k for _, o in cfgs for k, _ in o})
-    defaults = {"tc_lean_epi": 1, "tc_rowstack": 1, "tc_xf_early": 1, "tc_prefetch": 4, "tc_ar": 1, "tc_ar_min_chunks": 1, "tc_ar_nres": 2, "tc_ar_min_wst": 3, "tc_xf_trunc": 1, "tc_res_tma": 1}
+    defaults = {"tc_prefetch": 4, "tc_xf_trunc": 1, "tc_seg_chunks": 4, "tc_block_n": 0, "xform": 1}
     net.ctx.forward(x)
     net.ctx.set_option("profile", 3)
     times = {t: {} for t, _ in cfgs}

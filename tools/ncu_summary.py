@@ -72,7 +72,8 @@ def traffic(path):
 
 
 def main(tag):
-    out = ["# ncu summaries, round %s (B200, `--clock-control none`)" % tag, ""]
+    out = ["# ncu summaries, round %s (`--clock-control none`)" % tag, ""]
+    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
     lp = os.path.join(ROOT, "gpurun_out", "%s_launches.csv" % tag)
     if not os.path.exists(lp):
         lp += ".gz"

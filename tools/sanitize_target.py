@@ -1,9 +1,8 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): 1 patch through CNN +
-post-processing (every k_conv_tc variant the plan uses -- plain, XF in-place transform, RT, two-source, HALO on every
-eligible layer -- and the tensor-core stem), device contours, the whole-image tile path on a small image, the packed
+post-processing (every k_conv_tc variant the plan uses -- plain, XF transform, residual, two-source, upsample -- and the
+tensor-core stem), device contours, the whole-image tile path on a small image, the packed
 table gather kernel, and a 300x200 synthetic map through the generic (large-map) flood.
-The default knobs put the residual units' conv3 on k_conv_ar and the grouped k x k layers on k_conv_rs (<3> in fast mode,
-<5> in original mode).  HVN_SAN_MODE=original runs the 270x270 / 5x5 variant of the CNN part only; HVN_SAN_CNN_ONLY=1 stops
+HVN_SAN_MODE=original runs the 270x270 / 5x5 variant of the CNN part only; HVN_SAN_CNN_ONLY=1 stops
 the fast-mode run after the CNN + post-processing pass; HVN_SAN_REFEREE=1 adds the CUDA-core referee."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -14,7 +13,6 @@ from hover_net_b200.models.hovernet.net_desc import create_model
 if os.environ.get("HVN_SAN_MODE") == "original":
     net = create_model(mode="original", nr_types=5)
     net.load_state_dict(synth.make_state_dict("original", 5, 0))
-    net.ctx.set_option("tc_halo", 2)
     x = synth.make_patches(1, 270, seed=1)
     pred, inst, tab, n = net.ctx.forward_postproc(x)
     print("tc path (original) ok", int(n[0]), bool(np.isfinite(pred).all()))
@@ -22,11 +20,10 @@ if os.environ.get("HVN_SAN_MODE") == "original":
     sys.exit(0)
 net = create_model(mode="fast", nr_types=6)
 net.load_state_dict(synth.make_state_dict("fast", 6, 0))
-net.ctx.set_option("tc_halo", 2)
 x = synth.make_patches(1, 256, seed=1)
 pred, inst, tab, n = net.ctx.forward_postproc(x)
 print("tc path ok", int(n[0]))
-if os.environ.get("HVN_SAN_CNN_ONLY"):   # the kernels of csrc/conv_tc.cu only (k_conv_tc variants, k_conv_ar, k_conv_rs<3>, stem)
+if os.environ.get("HVN_SAN_CNN_ONLY"):   # the kernels of csrc/conv_tc.cu only (k_conv_tc variants, stem)
     net.ctx.close()
     sys.exit(0)
 pm = synth.synth_pred_map(164, 164, 6, 0)

@@ -4,7 +4,7 @@
 //   mode 1  unicast, the two CTAs of a cluster fetch the SAME tile (32 KB each)
 //   mode 2  multicast, each CTA of a cluster fetches half a tile (16 KB) and multicasts it to both: 32 KB land per CTA
 //   mode 3  unicast from a 4 GB buffer (HBM)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -o tools/tma_bw_probe tools/tma_bw_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -o tools/tma_bw_probe tools/tma_bw_probe.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
