@@ -53,6 +53,17 @@ def _ptr(a):
     return ctypes.c_void_p(int(a))  # raw address (device pointer or pinned host)
 
 
+def _as_ids(a):
+    """Instance map as C-contiguous int32; ids that int32 cannot hold are an error, never wrapped."""
+    a = np.asarray(a)
+    if a.dtype == np.int32:
+        return np.ascontiguousarray(a)
+    b = np.ascontiguousarray(a, dtype=np.int32)
+    if not np.array_equal(b, a):
+        raise ValueError("instance ids must be integers that fit in int32")
+    return b
+
+
 class Context:
     """One libhvn context (one device, one stream)."""
 
@@ -196,6 +207,50 @@ class Context:
                                        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
         check(L.hvn_contours_dev(self._h, _ptr(d_inst), _ptr(d_table), _ptr(d_nrows), n, H, W, int(max_rows), _ptr(d_pts),
                                  int(pts_cap), _ptr(d_offs)))
+
+    _PAIRS_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                   ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+
+    def inst_pairs(self, true, pred=None, cap=None):
+        """Contingency table of instance maps true/pred [H,W] or [n,H,W] (ids >= 0, 0 = background; pred None = all
+        zero).  Returns (rows [total,3] int64 (t, p, count), offs [n+1] int64): the rows of map m are
+        rows[offs[m]:offs[m+1]], every (t, p) with t > 0 or p > 0 that occurs, sorted by (t, p)."""
+        t = _as_ids(true)
+        p = None if pred is None else _as_ids(pred)
+        if t.ndim == 2:
+            t = t[None]
+            p = None if p is None else p[None]
+        if p is not None and p.shape != t.shape:
+            raise ValueError("true and pred shapes differ: %s vs %s" % (t.shape, p.shape))
+        n, H, W = t.shape
+        if cap is None:
+            cap = max(1024, n * H * W // 64)
+        L = lib()
+        L.hvn_inst_pairs.argtypes = self._PAIRS_ARGS
+        for _attempt in range(2):
+            rows = np.empty((cap, 3), dtype=np.int64)
+            offs = np.zeros((n + 1,), dtype=np.int64)
+            rc = L.hvn_inst_pairs(self._h, _ptr(t), _ptr(p), n, H, W, _ptr(rows), int(cap), _ptr(offs))
+            if rc == -4:  # HVN_ERR_CAPACITY: retry with the exact size
+                cap = int(offs[-1])
+                continue
+            check(rc)
+            rows = rows[: int(offs[-1])]
+            m = np.repeat(np.arange(n), np.diff(offs))
+            return rows[np.lexsort((rows[:, 1], rows[:, 0], m))], offs
+        raise HvnError(-4, "inst_pairs: capacity retries exhausted")
+
+    def inst_pairs_dev(self, d_true, d_pred, n, H, W, d_pairs, cap, d_offs):
+        """Device-pointer variant (d_pred may be None).  Returns False on HVN_ERR_CAPACITY (offs is valid on the
+        device then: retry with cap >= offs[n]), True on success; raises on any other error."""
+        L = lib()
+        L.hvn_inst_pairs_dev.argtypes = self._PAIRS_ARGS
+        rc = L.hvn_inst_pairs_dev(self._h, _ptr(d_true), _ptr(d_pred), int(n), int(H), int(W), _ptr(d_pairs),
+                                  int(cap), _ptr(d_offs))
+        if rc == -4:
+            return False
+        check(rc)
+        return True
 
     def tile_grid(self, H, W, patch_in):
         r, c = ctypes.c_int(), ctypes.c_int()

@@ -18,6 +18,7 @@ SOURCES = [
     ("postproc.cu", ["-fmad=false"]),
     ("contour.cu", []),
     ("tile.cu", []),
+    ("stats.cu", []),
 ]
 
 

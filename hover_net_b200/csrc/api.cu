@@ -6,6 +6,7 @@
 #include "../../include/hvn.h"
 #include "cnn.h"
 #include "postproc.h"
+#include "stats.h"
 #include "tile.h"
 
 using namespace hvn;
@@ -19,6 +20,7 @@ struct hvn_ctx {
     Arena pp_arena;                // post-processing workspace
     Arena io_arena;                // staging for the host-pointer entry points
     Arena tile_arena;              // patch / output batches of the tile path
+    Arena stats_arena;             // pair-table workspace of hvn_inst_pairs*
     int chunk = 0;
     int profile = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -89,6 +91,7 @@ void hvn_destroy(hvn_ctx *c) {
     c->pp_arena.release();
     c->io_arena.release();
     c->tile_arena.release();
+    c->stats_arena.release();
     for (auto &e : c->ev) cudaEventDestroy(e);
     for (auto &e : c->tev) cudaEventDestroy(e);
     cudaStreamDestroy(c->stream);
@@ -461,6 +464,70 @@ int hvn_infer_tile(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, i
             HVN_CUDA(cudaStreamSynchronize(c->stream));
         }
     }
+    API_END
+}
+
+// ---------------------------------------------------------------------------------------------------
+static void check_pairs_args(const int32_t *tru, const int64_t *pairs, int64_t cap, const int64_t *offs, int n, int H,
+                             int W) {
+    HVN_CHECK(tru && offs && (pairs || cap == 0), HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && cap >= 0, HVN_ERR_INVALID, "bad shape");
+    HVN_CHECK((long long)H * W <= 0x7fffffffll, HVN_ERR_INVALID, "map larger than 2^31 - 1 pixels");
+}
+static void check_pairs_result(int err, long long total, int64_t cap) {
+    HVN_CHECK(!err, HVN_ERR_INVALID, "negative instance id");
+    HVN_CHECK(total <= cap, HVN_ERR_CAPACITY,
+              "pair table too small: " + std::to_string(total) + " pairs, cap=" + std::to_string(cap));
+}
+
+int hvn_inst_pairs_dev(hvn_ctx *c, const int32_t *tru, const int32_t *pred, int n, int H, int W, int64_t *pairs,
+                       int64_t cap, int64_t *offs) {
+    API_BEGIN
+    use(c);
+    check_pairs_args(tru, pairs, cap, offs, n, H, W);
+    PairWork w;
+    inst_pairs_count(c->stats_arena, c->stream, tru, pred, n, H, W, (long long *)offs, w);
+    inst_pairs_emit(c->stream, w, (long long *)pairs, cap);
+    int err = 0;
+    long long total = 0;
+    HVN_CUDA(cudaMemcpyAsync(&err, w.err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(&total, offs + n, sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    check_pairs_result(err, total, cap);
+    API_END
+}
+
+int hvn_inst_pairs(hvn_ctx *c, const int32_t *tru, const int32_t *pred, int n, int H, int W, int64_t *pairs,
+                   int64_t cap, int64_t *offs) {
+    API_BEGIN
+    use(c);
+    check_pairs_args(tru, pairs, cap, offs, n, H, W);
+    const size_t px = (size_t)n * H * W;
+    c->io_arena.reset();
+    c->io_arena.reserve(px * 4 * (pred ? 2 : 1) + (size_t)(n + 1) * 8 + 4096);
+    int32_t *d_t = c->io_arena.take<int32_t>(px);
+    int32_t *d_p = pred ? c->io_arena.take<int32_t>(px) : nullptr;
+    long long *d_offs = c->io_arena.take<long long>((size_t)n + 1);
+    HVN_CUDA(cudaMemcpyAsync(d_t, tru, px * 4, cudaMemcpyHostToDevice, c->stream));
+    if (pred) HVN_CUDA(cudaMemcpyAsync(d_p, pred, px * 4, cudaMemcpyHostToDevice, c->stream));
+    PairWork w;
+    inst_pairs_count(c->stats_arena, c->stream, d_t, d_p, n, H, W, d_offs, w);
+    int err = 0;
+    HVN_CUDA(cudaMemcpyAsync(&err, w.err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(offs, d_offs, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    const long long total = offs[n];
+    check_pairs_result(err, total, cap);
+    if (total == 0) return HVN_OK;
+    // the maps are no longer needed: the staging arena now holds the rows
+    c->io_arena.reset();
+    c->io_arena.reserve((size_t)total * 24 + (size_t)(n + 1) * 8 + 1024);
+    long long *d_pairs = c->io_arena.take<long long>((size_t)total * 3);
+    w.offs = c->io_arena.take<long long>((size_t)n + 1);
+    HVN_CUDA(cudaMemcpyAsync(w.offs, offs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    inst_pairs_emit(c->stream, w, d_pairs, total);
+    HVN_CUDA(cudaMemcpyAsync(pairs, d_pairs, (size_t)total * 24, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
     API_END
 }
 

@@ -105,6 +105,21 @@ def synth_instances(h, w, seed=0, density=1.0 / 900.0, rmin=6.0, rmax=14.0):
     return inst
 
 
+def tiled_instances(h, w, block=256, seed=0, n_unique=16, density=1.0 / 900.0):
+    """int32 [h,w] instance map of seeded block x block `synth_instances` tiles (n_unique distinct ones, drawn in a
+    seeded order), every tile's ids offset so that all ids are distinct.  Fast for large maps."""
+    rng = np.random.default_rng(5000 + seed)
+    blocks = [synth_instances(block, block, seed=seed * 1000 + k, density=density) for k in range(n_unique)]
+    out = np.zeros((h, w), dtype=np.int32)
+    nid = 0
+    for y in range(0, h, block):
+        for x in range(0, w, block):
+            b = blocks[int(rng.integers(n_unique))][: h - y, : w - x]
+            out[y : y + b.shape[0], x : x + b.shape[1]] = np.where(b > 0, b + nid, 0)
+            nid += int(b.max())
+    return out
+
+
 def synth_pred_map(h, w, nr_types=None, seed=0, **kw):
     """float32 [h,w,C] pred map like `infer_step` output: [tp?, np_prob, hv_x, hv_y]."""
     rng = np.random.default_rng(3000 + seed)

@@ -154,6 +154,19 @@ int hvn_pack_tables_dev(hvn_ctx *ctx, const int64_t *table_dev, const int32_t *n
                         int64_t *packed_dev, int64_t cap_rows, int32_t *offs_dev);
 int hvn_get_stream(hvn_ctx *ctx, void **cuda_stream);
 
+/* ---- instance statistics (reference metrics/stats_utils.py, compute_stats.py): contingency table of two
+ * instance maps.  true/pred int32 [n_maps,H,W], ids >= 0, 0 = background; pred may be NULL (all zero, which gives
+ * the ids and areas of `true`).  pairs [cap,3] int64 (t, p, count) for every (t, p) with t > 0 or p > 0 that occurs,
+ * count > 0 (the (t, 0) and (0, p) rows are the parts that overlap background, so areas are row / column sums);
+ * rows of map m are [offs[m], offs[m+1]), order within a map unspecified.  offs [n_maps+1] int64.
+ * HVN_ERR_CAPACITY when offs[n_maps] > cap (offs valid, no rows written); HVN_ERR_INVALID on a negative id.
+ * n_maps <= 65535, H*W < 2^31.  Device workspace (context-owned, grow-only): 12 B per pixel of 8x128 tiles plus
+ * 12 * next_pow2(2*H*W) B per map.  Both variants synchronise the context stream to report the status. */
+int hvn_inst_pairs(hvn_ctx *ctx, const int32_t *true_host, const int32_t *pred_host, int n_maps, int H, int W,
+                   int64_t *pairs_host, int64_t cap, int64_t *offs_host);
+int hvn_inst_pairs_dev(hvn_ctx *ctx, const int32_t *true_dev, const int32_t *pred_dev, int n_maps, int H, int W,
+                       int64_t *pairs_dev, int64_t cap, int64_t *offs_dev);
+
 /* ---- device memory / stream helpers for callers without a CUDA binding of their own. */
 int hvn_malloc(hvn_ctx *ctx, size_t bytes, void **dev_ptr);
 int hvn_free(hvn_ctx *ctx, void *dev_ptr);
