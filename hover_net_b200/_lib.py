@@ -53,6 +53,17 @@ def _ptr(a):
     return ctypes.c_void_p(int(a))  # raw address (device pointer or pinned host)
 
 
+PRECISIONS = {"highest": 0, "high": 1}
+
+
+def precision_code(precision):
+    """"highest" -> 0, "high" -> 1 (libhvn option "precision"); anything else is a ValueError, raised before any
+    device is touched."""
+    if precision not in PRECISIONS:
+        raise ValueError("precision must be one of %s, got %r" % (sorted(PRECISIONS), precision))
+    return PRECISIONS[precision]
+
+
 def _as_ids(a):
     """Instance map as C-contiguous int32; ids that int32 cannot hold are an error, never wrapped."""
     a = np.asarray(a)
@@ -65,18 +76,24 @@ def _as_ids(a):
 
 
 class Context:
-    """One libhvn context (one device, one stream)."""
+    """One libhvn context (one device, one stream).  precision: "highest" (default; fp16 hi + lo operands, three
+    products per MAC) or "high" (hi only, one fp16 product per MAC -- TF32-class operand precision); model contexts
+    only, set before any weights are finalised."""
 
-    def __init__(self, device=0, mode=None, nr_types=None):
+    def __init__(self, device=0, mode=None, nr_types=None, precision="highest"):
+        code = precision_code(precision)
         self._h = ctypes.c_void_p()
         L = lib()
         if mode is None:
             check(L.hvn_create_postproc(int(device), ctypes.byref(self._h)))
         else:
             check(L.hvn_create(int(device), mode.encode(), int(nr_types or 0), ctypes.byref(self._h)))
+            if code:
+                self.set_option("precision", code)
         self.device = int(device)
         self.mode = mode
         self.nr_types = nr_types
+        self.precision = precision
         for kv in os.environ.get("HVN_OPTS", "").split(","):  # development knobs: HVN_OPTS="key=value,..."
             if "=" in kv and mode is not None:
                 k, v = kv.split("=")

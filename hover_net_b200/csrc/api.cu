@@ -153,6 +153,15 @@ int hvn_set_option(hvn_ctx *c, const char *key, int64_t value) {
             if (c->model->finalized) c->model->finalize();  // re-derives the BN shifts / head weights; plans are rebuilt
         }
     }
+    else if (k == "precision") {
+        HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+        HVN_CHECK(value == 0 || value == 1, HVN_ERR_INVALID, "precision must be 0 (highest) or 1 (high)");
+        if (c->model->precision != (int)value) {
+            HVN_CUDA(cudaStreamSynchronize(c->stream));
+            c->model->precision = (int)value;
+            if (c->model->finalized) c->model->finalize();  // weight planes re-derived (lo dropped / restored); plans rebuilt
+        }
+    }
     else if (k == "profile") { c->profile = (int)value; if (c->model) c->model->profile_ops = value >= 3 ? 2 : (value >= 2 ? 1 : 0); }
     else throw Error(HVN_ERR_INVALID, "unknown option " + k);
     API_END
@@ -162,6 +171,8 @@ int64_t hvn_get_counter(const hvn_ctx *c, const char *key) {
     if (!c || !key) return -1;
     std::string k = key;
     if (k == "act_shift") return c->model ? c->model->act_shift : 0;
+    if (k == "precision") return c->model ? c->model->precision : 0;
+    if (k == "plan_bytes") return c->model ? (int64_t)c->model->last_plan_bytes : 0;
     if (k == "kernel_launches") return (c->model ? c->model->kernel_launches : 0) + c->pp_launches;
     if (k == "tc_launches") return c->model ? c->model->tc_launches : 0;
     if (k == "pp_launches") return c->pp_launches;

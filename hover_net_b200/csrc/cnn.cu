@@ -144,6 +144,17 @@ static int weight_exponent(float mx) {
     return 14 - ex;
 }
 
+// hi (and, in precision "highest", lo) weight planes -> device
+void Model::upload_planes(ConvWeights &cw, const std::vector<__half> &hi, const std::vector<__half> &lo) {
+    cw.hi = dalloc<__half>(hi.size(), wallocs_, false);
+    HVN_CUDA(cudaMemcpy(cw.hi, hi.data(), hi.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    cw.lo = nullptr;
+    if (precision == 0) {
+        cw.lo = dalloc<__half>(lo.size(), wallocs_, false);
+        HVN_CUDA(cudaMemcpy(cw.lo, lo.data(), lo.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    }
+}
+
 // OIHW fp32 -> [tap][cout][cin_pad] split fp16 (grouped convs become block-diagonal dense)
 void Model::make_conv(const std::string &name, int groups) {
     const ParamSpec &s = spec[index.at(name)];
@@ -172,10 +183,7 @@ void Model::make_conv(const std::string &name, int groups) {
                 lo[d] = l;
             }
     }
-    cw.hi = dalloc<__half>(n, wallocs_, false);
-    cw.lo = dalloc<__half>(n, wallocs_, false);
-    HVN_CUDA(cudaMemcpy(cw.hi, hi.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
-    HVN_CUDA(cudaMemcpy(cw.lo, lo.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
+    upload_planes(cw, hi, lo);
     float *d_osc = dalloc<float>(O, wallocs_, false);
     HVN_CUDA(cudaMemcpy(d_osc, osc.data(), O * sizeof(float), cudaMemcpyHostToDevice));
     cw.oscale = d_osc;
@@ -207,10 +215,7 @@ void Model::make_conv_concat(const std::string &key, const std::string &name1, c
             lo[(size_t)o * cw.cin_pad + i] = __float2half_rn(v - __half2float(h));
         }
     }
-    cw.hi = dalloc<__half>(n, wallocs_, false);
-    cw.lo = dalloc<__half>(n, wallocs_, false);
-    HVN_CUDA(cudaMemcpy(cw.hi, hi.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
-    HVN_CUDA(cudaMemcpy(cw.lo, lo.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
+    upload_planes(cw, hi, lo);
     float *d_osc = dalloc<float>(O, wallocs_, false);
     HVN_CUDA(cudaMemcpy(d_osc, osc.data(), O * sizeof(float), cudaMemcpyHostToDevice));
     cw.oscale = d_osc;
@@ -256,6 +261,7 @@ void Model::finalize() {
     wallocs_.clear();
     conv_.clear(); bn_.clear(); head_w_.clear(); head_b_.clear();
     HVN_CHECK(act_shift >= 0 && act_shift <= 48, -1, "act_shift out of range (0..48)");
+    HVN_CHECK(precision == 0 || precision == 1, -1, "precision must be 0 (highest) or 1 (high)");
     if (!d_flag_) {
         HVN_CUDA(cudaMalloc((void **)&d_flag_, sizeof(unsigned int)));
         HVN_CUDA(cudaMemset(d_flag_, 0, sizeof(unsigned int)));
@@ -268,11 +274,20 @@ void Model::finalize() {
         if (n == "conv0./.weight") {
             const auto &w = hostp(n);  // OIHW [64][3][7][7] -> [ky][kx][ch][64]
             std::vector<float> t(7 * 7 * 3 * 64);
-            for (int o = 0; o < 64; ++o)
+            for (int o = 0; o < 64; ++o) {
+                // precision "high": the CUDA-core stem multiplies by the same fp16 weights as the tensor-core one,
+                // fp16(w * 2^e) * 2^-e with the channel's exponent (exact)
+                float mx = 0.f;
+                for (int j = 0; j < 147; ++j) mx = std::max(mx, std::fabs(w[(size_t)o * 147 + j]));
+                const int e = weight_exponent(mx);
                 for (int ch = 0; ch < 3; ++ch)
                     for (int ky = 0; ky < 7; ++ky)
-                        for (int kx = 0; kx < 7; ++kx)
-                            t[((ky * 7 + kx) * 3 + ch) * 64 + o] = w[((o * 3 + ch) * 7 + ky) * 7 + kx];
+                        for (int kx = 0; kx < 7; ++kx) {
+                            float v = w[((o * 3 + ch) * 7 + ky) * 7 + kx];
+                            if (precision == 1) v = std::ldexp(__half2float(__float2half_rn(std::ldexp(v, e))), -e);
+                            t[((ky * 7 + kx) * 3 + ch) * 64 + o] = v;
+                        }
+            }
             conv0_w_ = dalloc<float>(t.size(), wallocs_, false);
             HVN_CUDA(cudaMemcpy(conv0_w_, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
             {   // tensor-core stem operand: [64 cout][192 k] split fp16, k = ky * 24 + kx * 3 + ch, zeros elsewhere
@@ -295,10 +310,7 @@ void Model::finalize() {
                                 lo[d] = __float2half_rn(v - __half2float(h));
                             }
                 }
-                cw.hi = dalloc<__half>(hi.size(), wallocs_, false);
-                cw.lo = dalloc<__half>(lo.size(), wallocs_, false);
-                HVN_CUDA(cudaMemcpy(cw.hi, hi.data(), hi.size() * sizeof(__half), cudaMemcpyHostToDevice));
-                HVN_CUDA(cudaMemcpy(cw.lo, lo.data(), lo.size() * sizeof(__half), cudaMemcpyHostToDevice));
+                upload_planes(cw, hi, lo);
                 float *d_osc = dalloc<float>(64, wallocs_, false);
                 HVN_CUDA(cudaMemcpy(d_osc, osc.data(), 64 * sizeof(float), cudaMemcpyHostToDevice));
                 cw.oscale = d_osc;
@@ -374,7 +386,8 @@ __global__ void k_cmp_split(const __half *ah, const __half *al, const __half *bh
         int x = (int)(t % w); t /= w;
         int y = (int)(t % h); int n = (int)(t / h);
         long long o = n * sN + (long long)y * sH + (long long)x * sW + ch;
-        float va = __half2float(ah[o]) + __half2float(al[o]), vb = __half2float(bh[o]) + __half2float(bl[o]);
+        float va = __half2float(ah[o]), vb = __half2float(bh[o]);
+        if (al) { va += __half2float(al[o]); vb += __half2float(bl[o]); }  // single-plane tensors: hi only
         float d = fabsf(va - vb);
         if (!(d == d)) d = 3.0e38f;
         md = fmaxf(md, d); mr = fmaxf(mr, fabsf(vb));
@@ -394,8 +407,9 @@ void Model::selftest_conv(const Op &op, cudaStream_t s) {
     }
     if (op.cp.out_split.hi) {
         size_t n = (size_t)B * op.cp.out_split.sN;
-        a.out_split.hi = (__half *)dz(n * 2); a.out_split.lo = (__half *)dz(n * 2);
-        b.out_split.hi = (__half *)dz(n * 2); b.out_split.lo = (__half *)dz(n * 2);
+        const bool lo = op.cp.out_split.lo != nullptr;
+        a.out_split.hi = (__half *)dz(n * 2); a.out_split.lo = lo ? (__half *)dz(n * 2) : nullptr;
+        b.out_split.hi = (__half *)dz(n * 2); b.out_split.lo = lo ? (__half *)dz(n * 2) : nullptr;
     }
     unsigned int *d_out = (unsigned int *)dz(16);
     const bool trace = getenv("HVN_TRACE") != nullptr;
@@ -437,7 +451,9 @@ namespace {
 SplitRef sview(const SplitRef &b, int y0, int x0, int h, int w, int c0, int c) {
     SplitRef v = b;
     long long off = (long long)y0 * b.sH + (long long)x0 * b.sW + c0;
-    v.hi += off; v.lo += off; v.h = h; v.w = w; v.c = c;
+    v.hi += off;
+    if (v.lo) v.lo += off;
+    v.h = h; v.w = w; v.c = c;
     return v;
 }
 RawRef rview(const RawRef &b, int y0, int x0, int h, int w, int c0, int c) {
@@ -464,8 +480,8 @@ Plan &Model::plan(int B, int H, int W) {
         SplitRef r;
         size_t n = (size_t)B * h * w * c;
         r.hi = dalloc<__half>(n, P.allocs, true);
-        r.lo = dalloc<__half>(n, P.allocs, true);
-        P.bytes += 2 * n * sizeof(__half);
+        r.lo = precision == 0 ? dalloc<__half>(n, P.allocs, true) : nullptr;  // "high": one plane
+        P.bytes += (precision == 0 ? 2 : 1) * n * sizeof(__half);
         r.sN = (long long)h * w * c; r.sH = w * c; r.sW = c; r.h = h; r.w = w; r.c = c;
         r.flag = d_flag_;
         return r;
@@ -689,12 +705,16 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
     std::vector<Rec> recs;
     if (profile_ops) { class_ms.clear(); class_flops.clear(); class_launches.clear(); }
     last_flops = 0;
+    last_plan_bytes = 0;
+    const Plan *last_plan = nullptr;
     if (conv_path == 2 || profile_ops >= 2) debug_log.clear();
 
     for (int b0 = 0; b0 < B; b0 += chunk) {
         int bc = std::min(chunk, B - b0);
         Plan &P = plan(bc, H, W);
         last_flops += P.flops;
+        if (&P != last_plan) last_plan_bytes += P.bytes;  // a tail chunk runs a second, smaller plan
+        last_plan = &P;
         int prev_stream = 0;
         bool forked[3] = {true, false, false};
         for (auto &op : P.ops) {

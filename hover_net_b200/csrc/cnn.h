@@ -74,6 +74,11 @@ class Model {
     // is unchanged (powers of two are exact) while the representable range grows to 65504 * 2^s.  0 by default; raise
     // it when a forward reports HVN_ERR_RANGE (the Python binding retries with +6 automatically).
     int act_shift = 0;
+    // Convolution operand precision.  0 "highest": activations that feed a convolution and its weights are stored as
+    // fp16 hi + lo and every MAC forms hi*hi + hi*lo + lo*hi.  1 "high": hi planes only (no lo is allocated), one fp16
+    // product per MAC -- the operand precision of TF32.  Accumulation, residual sums, BN and heads stay fp32 in both.
+    // Weights are re-finalised on a change.
+    int precision = 0;
     // true if the last forward() stored a value outside the fp16 range (valid after the stream was synchronised)
     bool range_overflow() const { return h_flag_ && *h_flag_ != 0; }
     void reset_range_flag(cudaStream_t s);  // after the host has seen (and reported) an overflow
@@ -92,6 +97,7 @@ class Model {
     std::map<std::string, double> class_ms, class_flops;
     std::map<std::string, long long> class_launches;
     double last_flops = 0;  // algorithmic 2*MACs of the last forward()
+    size_t last_plan_bytes = 0;  // device bytes of the plan(s) the last forward() ran
     std::string debug_log;  // conv_path == 2: per-layer wgmma-vs-referee report of the last forward()
     void selftest_conv(const Op &op, cudaStream_t s);
 
@@ -114,6 +120,7 @@ class Model {
     void make_conv(const std::string &name, int groups);
     void make_conv_concat(const std::string &key, const std::string &name1, const std::string &name2);
     void make_bn(const std::string &prefix);
+    void upload_planes(ConvWeights &cw, const std::vector<__half> &hi, const std::vector<__half> &lo);
     template <typename T> T *dalloc(size_t n, std::vector<void *> &owner, bool zero);
 };
 

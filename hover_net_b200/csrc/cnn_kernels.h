@@ -42,6 +42,7 @@ struct TcPlan {
     int tiles_x = 0, tiles_y = 0;
     int block_n = 0;
     int flat = 0;                // 1x1 stride-1 dense view: M flattened over B*H*W
+    int single = 0;              // precision "high": hi planes only, one wgmma per K=16 step (no lo tensor maps)
 };
 bool tc_plan(const ConvParams &P, TcPlan &plan);
 void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s);

@@ -15,6 +15,13 @@ __device__ __forceinline__ void split_f32(float x, __half &hi, __half &lo, unsig
 
 __device__ __forceinline__ float join_f16(__half hi, __half lo) { return __half2float(hi) + __half2float(lo); }
 
+// Single-plane tensors (precision "high": SplitRef::lo == nullptr) store only hi = fp16_rn(x) -- the same hi, with the same
+// range check and clamp, as split_f32 -- and read back as hi alone.
+__device__ __forceinline__ __half hi_f32(float x, unsigned int *flag = nullptr) {
+    if (flag && fabsf(x) > 65504.f) *flag = 1u;
+    return __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
+}
+
 // Four values at once with the packed conversions (one F2FP per pair): same roundings as split_f32.
 // NONNEG: the inputs are already >= 0 (post-ReLU), so only the upper clamp is needed.
 template <bool NONNEG = false>
@@ -32,6 +39,14 @@ __device__ __forceinline__ void split4_f32(const float t[4], uint2 &hi, uint2 &l
     const __half2 l01 = __floats2half2_rn(x[0] - f01.x, x[1] - f01.y), l23 = __floats2half2_rn(x[2] - f23.x, x[3] - f23.y);
     hi = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
     lo = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
+}
+
+// hi of split4_f32<true> alone: fp16_rn of four values >= 0, clamped at 65504 (single-plane XF tiles; the caller keeps
+// the running maximum for the range guard)
+__device__ __forceinline__ uint2 hi4_f32_nonneg(const float t[4]) {
+    const __half2 h01 = __floats2half2_rn(fminf(t[0], 65504.f), fminf(t[1], 65504.f));
+    const __half2 h23 = __floats2half2_rn(fminf(t[2], 65504.f), fminf(t[3], 65504.f));
+    return make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
 }
 
 // relu(y) split by TRUNCATION, for the XF transform warps whose instruction count paces the tensor core:
@@ -77,15 +92,16 @@ __device__ __forceinline__ void conv_epilogue4(const ConvParams &P, int n, int o
             long long so = n * P.skip.sN + (long long)Y * P.skip.sH + (long long)X * P.skip.sW + c;
             long long oo = n * P.out_split.sN + (long long)Y * P.out_split.sH + (long long)X * P.out_split.sW + c;
             const __half2 *sh = reinterpret_cast<const __half2 *>(P.skip.hi + so);
-            const __half2 *sl = reinterpret_cast<const __half2 *>(P.skip.lo + so);
-            __half2 h01 = sh[0], h23 = sh[1], l01 = sl[0], l23 = sl[1];
+            const __half2 zero = __float2half2_rn(0.f);
+            const __half2 *sl = P.skip.lo ? reinterpret_cast<const __half2 *>(P.skip.lo + so) : nullptr;
+            __half2 h01 = sh[0], h23 = sh[1], l01 = sl ? sl[0] : zero, l23 = sl ? sl[1] : zero;
             float t[4] = {v[0] + join_f16(h01.x, l01.x), v[1] + join_f16(h01.y, l01.y),
                           v[2] + join_f16(h23.x, l23.x), v[3] + join_f16(h23.y, l23.y)};
             __half oh[4], ol[4];
 #pragma unroll
             for (int i = 0; i < 4; ++i) split_f32(t[i], oh[i], ol[i], P.out_split.flag);
             *reinterpret_cast<uint2 *>(P.out_split.hi + oo) = *reinterpret_cast<uint2 *>(oh);
-            *reinterpret_cast<uint2 *>(P.out_split.lo + oo) = *reinterpret_cast<uint2 *>(ol);
+            if (P.out_split.lo) *reinterpret_cast<uint2 *>(P.out_split.lo + oo) = *reinterpret_cast<uint2 *>(ol);
         }
     } else if (P.out_split.hi) {
         float t[4] = {v[0], v[1], v[2], v[3]};
@@ -103,7 +119,7 @@ __device__ __forceinline__ void conv_epilogue4(const ConvParams &P, int n, int o
         for (int i = 0; i < 4; ++i) split_f32(t[i], oh[i], ol[i], P.out_split.flag);
         long long oo = n * P.out_split.sN + (long long)oy * P.out_split.sH + (long long)ox * P.out_split.sW + c;
         *reinterpret_cast<uint2 *>(P.out_split.hi + oo) = *reinterpret_cast<uint2 *>(oh);
-        *reinterpret_cast<uint2 *>(P.out_split.lo + oo) = *reinterpret_cast<uint2 *>(ol);
+        if (P.out_split.lo) *reinterpret_cast<uint2 *>(P.out_split.lo + oo) = *reinterpret_cast<uint2 *>(ol);
     }
 }
 
@@ -128,7 +144,7 @@ __device__ __forceinline__ void epi_prefetch(const ConvParams &P, int n, int oy,
             int Y = 2 * oy + (d >> 1), X = 2 * ox + (d & 1);
             long long so = n * P.skip.sN + (long long)Y * P.skip.sH + (long long)X * P.skip.sW + c;
             pre.h[d] = *reinterpret_cast<const uint2 *>(P.skip.hi + so);
-            pre.l[d] = *reinterpret_cast<const uint2 *>(P.skip.lo + so);
+            pre.l[d] = P.skip.lo ? *reinterpret_cast<const uint2 *>(P.skip.lo + so) : make_uint2(0u, 0u);
         }
     }
 }
@@ -137,7 +153,7 @@ __device__ __forceinline__ void store_split4(const SplitRef &o, long long off, c
     uint2 oh, ol;
     split4_f32(t, oh, ol, o.flag);
     *reinterpret_cast<uint2 *>(o.hi + off) = oh;
-    *reinterpret_cast<uint2 *>(o.lo + off) = ol;
+    if (o.lo) *reinterpret_cast<uint2 *>(o.lo + off) = ol;
 }
 
 // sc / sh: the BN scale / shift of channels c..c+3, loaded once per tile by the caller (they do not depend

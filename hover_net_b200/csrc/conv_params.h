@@ -2,6 +2,8 @@
 // convolution (conv_tc.cu).  Activations are NHWC.  A "split" tensor stores x as two fp16 planes
 // hi = fp16(x), lo = fp16(x - hi): x ~= hi + lo to ~2^-22 relative, which lets the tensor cores
 // reproduce fp32-grade products with three fp16 MMAs (hi*hi + hi*lo + lo*hi, fp32 accumulate).
+// Precision "high" keeps the hi plane alone (lo == nullptr, read as 0 and never written): one fp16 product per MAC,
+// the operand precision of TF32.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>

@@ -1,7 +1,8 @@
 // CUDA-core kernels of the CNN path (sm_90a):
 //   k_conv_ref   generic NHWC implicit-GEMM convolution in fp32 on split-fp16 operands.  It is the
 //                on-device referee for the wgmma kernel (same operands, same epilogue) and the
-//                executor for layers the tensor-core kernel does not take.
+//                executor for layers the tensor-core kernel does not take.  An absent `lo` plane
+//                (precision "high": activations and weights stored as hi only) reads as 0.
 //   k_conv0      7x7x3 -> 64 stem on the uint8 image (reference net_desc.py:27-35,103,115)
 //   k_bnrelu     BatchNorm(eval)+ReLU raw fp32 -> split (dense-unit preact / blk_bna, net_utils.py:98-99,135-142)
 //   k_head       1x1 64->out_ch + bias for every branch, softmax / argmax, concat to [B,h,w,C]
@@ -52,7 +53,7 @@ __global__ void __launch_bounds__(256) k_conv_ref(const ConvParams P) {
             float a4[4] = {0.f, 0.f, 0.f, 0.f}, b4[4] = {0.f, 0.f, 0.f, 0.f};
             if (inb) {
                 uint2 h = *reinterpret_cast<const uint2 *>(P.a.hi + aoff + c0 + kq);
-                uint2 l = *reinterpret_cast<const uint2 *>(P.a.lo + aoff + c0 + kq);
+                uint2 l = P.a.lo ? *reinterpret_cast<const uint2 *>(P.a.lo + aoff + c0 + kq) : make_uint2(0u, 0u);
                 const __half *hh = reinterpret_cast<const __half *>(&h);
                 const __half *ll = reinterpret_cast<const __half *>(&l);
 #pragma unroll
@@ -60,7 +61,7 @@ __global__ void __launch_bounds__(256) k_conv_ref(const ConvParams P) {
             }
             if (nvalid) {
                 uint2 h = *reinterpret_cast<const uint2 *>(P.w.hi + woff + c0 + kq);
-                uint2 l = *reinterpret_cast<const uint2 *>(P.w.lo + woff + c0 + kq);
+                uint2 l = P.w.lo ? *reinterpret_cast<const uint2 *>(P.w.lo + woff + c0 + kq) : make_uint2(0u, 0u);
                 const __half *hh = reinterpret_cast<const __half *>(&h);
                 const __half *ll = reinterpret_cast<const __half *>(&l);
 #pragma unroll
@@ -91,7 +92,7 @@ __global__ void __launch_bounds__(256) k_conv_ref(const ConvParams P) {
             float a4[4] = {0.f, 0.f, 0.f, 0.f}, b4[4] = {0.f, 0.f, 0.f, 0.f};
             if (inb) {
                 uint2 h = *reinterpret_cast<const uint2 *>(P.a2.hi + aoff + c0 + kq);
-                uint2 l = *reinterpret_cast<const uint2 *>(P.a2.lo + aoff + c0 + kq);
+                uint2 l = P.a2.lo ? *reinterpret_cast<const uint2 *>(P.a2.lo + aoff + c0 + kq) : make_uint2(0u, 0u);
                 const __half *hh = reinterpret_cast<const __half *>(&h);
                 const __half *ll = reinterpret_cast<const __half *>(&l);
 #pragma unroll
@@ -99,7 +100,7 @@ __global__ void __launch_bounds__(256) k_conv_ref(const ConvParams P) {
             }
             if (nvalid) {
                 uint2 h = *reinterpret_cast<const uint2 *>(P.w.hi + woff + c0 + kq);
-                uint2 l = *reinterpret_cast<const uint2 *>(P.w.lo + woff + c0 + kq);
+                uint2 l = P.w.lo ? *reinterpret_cast<const uint2 *>(P.w.lo + woff + c0 + kq) : make_uint2(0u, 0u);
                 const __half *hh = reinterpret_cast<const __half *>(&h);
                 const __half *ll = reinterpret_cast<const __half *>(&l);
 #pragma unroll
@@ -147,6 +148,8 @@ void launch_conv_ref(const ConvParams &P, cudaStream_t s) {
 // (8 shared loads per 64 FMAs; the per-pixel form it replaces issued 16 loads per 64).  The 7 input rows
 // of the segment are staged as floats already divided by 255 (the reference's own `imgs / 255.0`), zero
 // outside the image.  Accumulation order per output is (ky, kx, channel), as in the reference's direct sum.
+// Single-plane output (precision "high"): the staged inputs are rounded to fp16 and the host passes weights already
+// rounded to fp16 (under the per-channel exponent), so every product is the one k_conv0_tc forms, exact in fp32.
 constexpr int C0_PX = 128, C0_IN = (C0_PX + 6) * 3;
 __global__ void __launch_bounds__(128) k_conv0(const uint8_t *__restrict__ img, int B, int H, int W, int pad,
                                                const float *__restrict__ wgt /*[7][7][3][64]*/,
@@ -166,7 +169,7 @@ __global__ void __launch_bounds__(128) k_conv0(const uint8_t *__restrict__ img, 
         const int iy = oy + row - pad, ix = x0 + pxi - pad;
         float v = 0.f;
         if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = (float)im[((size_t)iy * W + ix) * 3 + ch] / 255.0f;
-        s_in[i] = v;
+        s_in[i] = out.lo ? v : __half2float(__float2half_rn(v));
     }
     __syncthreads();
     const int cg = t & 3, pq = t >> 2;      // 16-channel group, pixel quad
@@ -254,7 +257,7 @@ __global__ void __launch_bounds__(256) k_bnrelu(RawRef in, int B, const float *_
         for (int k = 0; k < 4; ++k) split_f32(tt[k], oh[k], ol[k], out.flag);
         long long oo = n * out.sN + (long long)y * out.sH + (long long)x * out.sW + c;
         *reinterpret_cast<uint2 *>(out.hi + oo) = *reinterpret_cast<uint2 *>(oh);
-        *reinterpret_cast<uint2 *>(out.lo + oo) = *reinterpret_cast<uint2 *>(ol);
+        if (out.lo) *reinterpret_cast<uint2 *>(out.lo + oo) = *reinterpret_cast<uint2 *>(ol);
     }
 }
 
@@ -282,7 +285,8 @@ __global__ void __launch_bounds__(256) k_up2_add(RawRef in, int B, SplitRef skip
         const float *ip = in.p + n * in.sN + (long long)(Y >> 1) * in.sH + (long long)(X >> 1) * in.sW + c;
         const float4 v0 = *reinterpret_cast<const float4 *>(ip), v1 = *reinterpret_cast<const float4 *>(ip + 4);
         const long long so = n * skip.sN + (long long)Y * skip.sH + (long long)X * skip.sW + c;
-        const uint4 sh = *reinterpret_cast<const uint4 *>(skip.hi + so), sl = *reinterpret_cast<const uint4 *>(skip.lo + so);
+        const uint4 sh = *reinterpret_cast<const uint4 *>(skip.hi + so);
+        const uint4 sl = skip.lo ? *reinterpret_cast<const uint4 *>(skip.lo + so) : make_uint4(0u, 0u, 0u, 0u);
         const __half *hh = reinterpret_cast<const __half *>(&sh), *ll = reinterpret_cast<const __half *>(&sl);
         const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
         __half oh8[8], ol8[8];
@@ -290,7 +294,7 @@ __global__ void __launch_bounds__(256) k_up2_add(RawRef in, int B, SplitRef skip
         for (int k = 0; k < 8; ++k) split_f32(v[k] + join_f16(hh[k], ll[k]), oh8[k], ol8[k], out.flag);
         const long long oo = n * out.sN + (long long)Y * out.sH + (long long)X * out.sW + c;
         *reinterpret_cast<uint4 *>(out.hi + oo) = *reinterpret_cast<uint4 *>(oh8);
-        *reinterpret_cast<uint4 *>(out.lo + oo) = *reinterpret_cast<uint4 *>(ol8);
+        if (out.lo) *reinterpret_cast<uint4 *>(out.lo + oo) = *reinterpret_cast<uint4 *>(ol8);
     }
 }
 
@@ -330,7 +334,7 @@ __global__ void __launch_bounds__(128) k_head(HeadParams P) {
         for (int o = 0; o < och; ++o) logit[o] = 0.f;
         for (int k = 0; k < 64; k += 4) {
             uint2 h = *reinterpret_cast<const uint2 *>(f.hi + fo + k);
-            uint2 l = *reinterpret_cast<const uint2 *>(f.lo + fo + k);
+            uint2 l = f.lo ? *reinterpret_cast<const uint2 *>(f.lo + fo + k) : make_uint2(0u, 0u);
             const __half *hh = reinterpret_cast<const __half *>(&h);
             const __half *ll = reinterpret_cast<const __half *>(&l);
             float a[4];

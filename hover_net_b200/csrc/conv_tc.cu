@@ -11,6 +11,9 @@
 // * Both operands land in 128B-swizzled shared memory and are read from there by wgmma (both K-major).  Per K=16 step
 //   three m64nNk16 instructions accumulate a_hi*w_hi + a_hi*w_lo + a_lo*w_hi in fp32 registers: fp32-grade products
 //   from fp16 tensor cores.
+// * Single-product variant (ONE, precision "high"): activations and weights are stored as hi only, the stages carry no
+//   lo tiles, and each K=16 step is one m64nNk16 a_hi*w_hi -- one fp16 product per MAC with fp32 accumulation, the
+//   operand precision of TF32.  The freed shared memory holds more stages; the epilogue stores hi only.
 // * Persistent CTAs (one per SM), warp-specialised: warp 0 = TMA producer; warpgroups 1 and 2 = consumers, each issuing
 //   the wgmma of 64 of the tile's 128 pixel rows over all BLOCK_N columns and running the fused epilogue (BN/ReLU/
 //   residual/upsample -> global) straight from its accumulator fragment.  A shared-memory ring of STAGES operand slots
@@ -128,6 +131,14 @@ __device__ __forceinline__ void mma_slice(float (&d)[N / 2], uint32_t a_hi, uint
     }
 }
 
+// One 64-channel K-slice of the single product a_hi*w_hi (precision "high")
+template <int N>
+__device__ __forceinline__ void mma_slice1(float (&d)[N / 2], uint32_t a_hi, uint32_t b_hi, bool zero) {
+    const uint64_t dah = wg_desc(a_hi), dbh = wg_desc(b_hi);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Wgmma<N>::mma(d, dah + 2 * k, dbh + 2 * k, (zero && k == 0) ? 0u : 1u);
+}
+
 struct TcGeom {
     int flat, bw, bh, tiles_x, tiles_y, tiles_m, tiles_n, kchunks, seg;
     int k1;  // > 0: K-slices [0,k1) come from the first source, [k1,kchunks) from the second (fused shortcut)
@@ -143,10 +154,22 @@ constexpr int CONS_WARPS = 8;
 constexpr int A_TILE_BYTES = 128 * 128;  // 128 rows x 64 fp16
 constexpr uint32_t RAW_TILE_BYTES = 128 * 64 * 4;
 
-template <int BLOCK_N> __host__ __device__ constexpr int tc_stage_bytes() { return 2 * A_TILE_BYTES + 2 * BLOCK_N * 128; }
-template <int BLOCK_N, int STAGES, bool XF> constexpr int tc_smem() {
-    return 1024 + STAGES * tc_stage_bytes<BLOCK_N>() + (XF ? 2 * (int)RAW_TILE_BYTES : 0) + 8 * (2 * STAGES + 4);
+// One operand stage: A then W tiles, hi planes (and, unless ONE, lo planes) -- [a_hi | a_lo | w_hi | w_lo]
+template <int BLOCK_N, bool ONE> __host__ __device__ constexpr int tc_stage_bytes() {
+    return (ONE ? 1 : 2) * (A_TILE_BYTES + BLOCK_N * 128);
 }
+template <int BLOCK_N, bool XF, bool ONE> constexpr int tc_smem(int stages) {
+    return 1024 + stages * tc_stage_bytes<BLOCK_N, ONE>() + (XF ? 2 * (int)RAW_TILE_BYTES : 0) + 8 * (2 * stages + 4);
+}
+// STAGES: as many operand slots as fit 227 KB beside the XF staging ring
+template <int BLOCK_N, bool XF, bool ONE> constexpr int tc_stages() {
+    int s = 1;
+    while (tc_smem<BLOCK_N, XF, ONE>(s + 1) <= SMEM_LIMIT) ++s;
+    return s;
+}
+static_assert(tc_stages<128, false, false>() == 3 && tc_stages<128, true, false>() == 2 && tc_stages<64, false, false>() == 4 &&
+                  tc_stages<64, true, false>() == 3 && tc_stages<32, false, false>() == 5,
+              "two-plane stage counts");
 
 // Output element offsets of one accumulator row (pixel); -1 = no such pixel.
 struct PixOff {
@@ -168,7 +191,12 @@ __device__ __forceinline__ PixOff pix_offsets(const ConvParams &P, bool valid, i
     return o;
 }
 
+template <bool ONE>
 __device__ __forceinline__ void store_split2(const SplitRef &o, long long off, float a, float b) {
+    if constexpr (ONE) {
+        *reinterpret_cast<__half2 *>(o.hi + off) = __halves2half2(hi_f32(a, o.flag), hi_f32(b, o.flag));
+        return;
+    }
     __half h0, l0, h1, l1;
     split_f32(a, h0, l0, o.flag);
     split_f32(b, h1, l1, o.flag);
@@ -178,7 +206,7 @@ __device__ __forceinline__ void store_split2(const SplitRef &o, long long off, f
 
 // Channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  Same operations, in the same order, as
 // epi_finish (conv_epilogue.cuh) on four channels.
-template <int MODE>
+template <int MODE, bool ONE>
 __device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, float2 s, float2 b) {
     if constexpr (MODE == EPI_RES) {
         const float2 r = *reinterpret_cast<const float2 *>(P.res.p + o.res + c);
@@ -190,26 +218,31 @@ __device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o
         for (int d = 0; d < 4; ++d) {
             const long long so = o.skip + (d >> 1) * P.skip.sH + (d & 1) * P.skip.sW + c;
             const __half2 sh = *reinterpret_cast<const __half2 *>(P.skip.hi + so);
-            const __half2 sl = *reinterpret_cast<const __half2 *>(P.skip.lo + so);
-            store_split2(P.out_split, o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c,
-                         v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
+            const long long oo = o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c;
+            if constexpr (ONE) {
+                store_split2<true>(P.out_split, oo, v0 + __half2float(sh.x), v1 + __half2float(sh.y));
+            } else {
+                const __half2 sl = *reinterpret_cast<const __half2 *>(P.skip.lo + so);
+                store_split2<false>(P.out_split, oo, v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
+            }
         }
     } else if (o.spl >= 0) {
         float t0 = v0, t1 = v1;
         if (P.scale) { t0 = t0 * s.x + b.x; t1 = t1 * s.y + b.y; }
         if (P.relu) { t0 = fmaxf(t0, 0.f); t1 = fmaxf(t1, 0.f); }
-        store_split2(P.out_split, o.spl + c, t0, t1);
+        store_split2<ONE>(P.out_split, o.spl + c, t0, t1);
     }
 }
 
-template <int BLOCK_N, int STAGES, int MODE, bool XF>
+template <int BLOCK_N, int STAGES, int MODE, bool XF, bool ONE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
           const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
           const __grid_constant__ CUtensorMap tm_a2_hi, const __grid_constant__ CUtensorMap tm_a2_lo,
           const ConvParams P, const TcGeom G) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    constexpr int STAGE_BYTES = tc_stage_bytes<BLOCK_N>();
+    constexpr int STAGE_BYTES = tc_stage_bytes<BLOCK_N, ONE>();
+    constexpr int PLANES = ONE ? 1 : 2;
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t raw_base = smem_base + STAGES * STAGE_BYTES;             // XF: 2-slot ring of raw fp32 [128][64] tiles
     const uint32_t bar_base = raw_base + (XF ? 2 * RAW_TILE_BYTES : 0u);
@@ -232,7 +265,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
     const int total_tiles = G.tiles_m * G.tiles_n;
     const int taps = P.w.taps;
     const int kiters = taps * G.kchunks;
-    const uint32_t tx_bytes = (uint32_t)(2 * (G.flat ? 128 : G.bw * G.bh) * 128 + 2 * BLOCK_N * 128);
+    const uint32_t tx_bytes = (uint32_t)(PLANES * ((G.flat ? 128 : G.bw * G.bh) * 128 + BLOCK_N * 128));
 
     if (warp == 0) {
         // ===================== TMA producer =====================
@@ -248,10 +281,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 if constexpr (XF) tma_prefetch_2d(&tm_a_hi, pf_it * 64, m0p);
                 else if (G.k1 > 0 && pf_it >= G.k1) {
                     tma_prefetch_2d(&tm_a2_hi, (pf_it - G.k1) * 64, m0p);
-                    tma_prefetch_2d(&tm_a2_lo, (pf_it - G.k1) * 64, m0p);
+                    if constexpr (!ONE) tma_prefetch_2d(&tm_a2_lo, (pf_it - G.k1) * 64, m0p);
                 } else {
                     tma_prefetch_2d(&tm_a_hi, pf_it * 64, m0p);
-                    tma_prefetch_2d(&tm_a_lo, pf_it * 64, m0p);
+                    if constexpr (!ONE) tma_prefetch_2d(&tm_a_lo, pf_it * 64, m0p);
                 }
                 if (++pf_it == kiters) { pf_it = 0; pf_tile += gridDim.x; }
             };
@@ -284,13 +317,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                     const uint32_t ph = (uint32_t)(it_global / STAGES) & 1u;
                     mbar_wait(empty_bar(s), ph ^ 1u);
                     const uint32_t sa = smem_base + s * STAGE_BYTES;
-                    const uint32_t a_hi = sa, a_lo = sa + A_TILE_BYTES, b_hi = sa + 2 * A_TILE_BYTES,
+                    const uint32_t a_hi = sa, a_lo = sa + A_TILE_BYTES, b_hi = sa + PLANES * A_TILE_BYTES,
                                    b_lo = b_hi + BLOCK_N * 128;
                     const int tap = it / G.kchunks, kc = it - tap * G.kchunks;
                     if constexpr (XF) {  // the A planes of the stage are written by the transform warps; weights land beside them
-                        mbar_expect_tx(full_bar(s), (uint32_t)(2 * BLOCK_N * 128));
+                        mbar_expect_tx(full_bar(s), (uint32_t)(PLANES * BLOCK_N * 128));
                         tma_3d(b_hi, &tm_w_hi, full_bar(s), kc * 64, tn * BLOCK_N, tap);
-                        tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
+                        if constexpr (!ONE) tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
                         continue;
                     }
                     mbar_expect_tx(full_bar(s), tx_bytes);
@@ -298,22 +331,22 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                         const int c2 = (kc - G.k1) * 64;
                         if (G.flat) {
                             tma_2d(a_hi, &tm_a2_hi, full_bar(s), c2, (int)m0);
-                            tma_2d(a_lo, &tm_a2_lo, full_bar(s), c2, (int)m0);
+                            if constexpr (!ONE) tma_2d(a_lo, &tm_a2_lo, full_bar(s), c2, (int)m0);
                         } else {
                             tma_4d(a_hi, &tm_a2_hi, full_bar(s), c2, x0 * P.a2_stride, y0 * P.a2_stride, n_img);
-                            tma_4d(a_lo, &tm_a2_lo, full_bar(s), c2, x0 * P.a2_stride, y0 * P.a2_stride, n_img);
+                            if constexpr (!ONE) tma_4d(a_lo, &tm_a2_lo, full_bar(s), c2, x0 * P.a2_stride, y0 * P.a2_stride, n_img);
                         }
                     } else if (G.flat) {
                         tma_2d(a_hi, &tm_a_hi, full_bar(s), kc * 64, (int)m0);
-                        tma_2d(a_lo, &tm_a_lo, full_bar(s), kc * 64, (int)m0);
+                        if constexpr (!ONE) tma_2d(a_lo, &tm_a_lo, full_bar(s), kc * 64, (int)m0);
                     } else {
                         const int ky = tap / P.w.kw, kx = tap - ky * P.w.kw;
                         const int cx = x0 * P.stride + kx - P.pad_l, cy = y0 * P.stride + ky - P.pad_t;
                         tma_4d(a_hi, &tm_a_hi, full_bar(s), kc * 64, cx, cy, n_img);
-                        tma_4d(a_lo, &tm_a_lo, full_bar(s), kc * 64, cx, cy, n_img);
+                        if constexpr (!ONE) tma_4d(a_lo, &tm_a_lo, full_bar(s), kc * 64, cx, cy, n_img);
                     }
                     tma_3d(b_hi, &tm_w_hi, full_bar(s), kc * 64, tn * BLOCK_N, tap);
-                    tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
+                    if constexpr (!ONE) tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
                 }
             }
         }
@@ -363,7 +396,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 uint8_t *a_hi = smem_gen + s * STAGE_BYTES, *a_lo = a_hi + A_TILE_BYTES;
                 // range guard: running maximum, tested once per tile (a flag store inside this loop cost the XF layers
                 // 40-60 %, measured).  128B swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7)).
-                if (G.xf_trunc) {  // truncating split (conv_epilogue.cuh): 4.5 instead of 7.25 instructions per element
+                if constexpr (ONE) {  // hi = fp16_rn(relu(y)): round to nearest -- truncation is only valid with a lo plane
+#pragma unroll
+                    for (int i = 0; i < XR; ++i) {
+                        const int row = rg + RG * i;
+                        if (128 % RG != 0 && i == XR - 1 && row >= 128) break;
+                        const float y4[4] = {fmaxf(v[i].x, 0.f), fmaxf(v[i].y, 0.f), fmaxf(v[i].z, 0.f), fmaxf(v[i].w, 0.f)};
+                        rmax = fmaxf(fmaxf(rmax, fmaxf(y4[0], y4[1])), fmaxf(y4[2], y4[3]));
+                        const int off = row * 128 + ((((l16 >> 1) ^ (row & 7))) << 4) + (l16 & 1) * 8;
+                        *reinterpret_cast<uint2 *>(a_hi + off) = hi4_f32_nonneg(y4);
+                    }
+                } else if (G.xf_trunc) {  // truncating split (conv_epilogue.cuh): 4.5 instead of 7.25 instructions per element
 #pragma unroll
                     for (int i = 0; i < XR; ++i) {
                         const int row = rg + RG * i;
@@ -418,9 +461,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 const int s = it_global % STAGES;
                 mbar_wait(full_bar(s), (uint32_t)(it_global / STAGES) & 1u);
                 const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;
-                const uint32_t sb = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES;
+                const uint32_t sb = smem_base + s * STAGE_BYTES + PLANES * A_TILE_BYTES;
                 wg_fence();
-                mma_slice<BLOCK_N>(acc, sa, sa + A_TILE_BYTES, sb, sb + BLOCK_N * 128, it % G.seg == 0);
+                if constexpr (ONE) mma_slice1<BLOCK_N>(acc, sa, sb, it % G.seg == 0);
+                else mma_slice<BLOCK_N>(acc, sa, sa + A_TILE_BYTES, sb, sb + BLOCK_N * 128, it % G.seg == 0);
                 wg_commit();
                 if ((it + 1) % G.seg == 0 || it + 1 == kiters) {   // segment complete: drain it into the fp32 sum
                     wg_wait<0>();
@@ -471,7 +515,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
                     if (po[h].raw >= 0 || po[h].spl >= 0)
-                        epi_finish2<MODE>(P, po[h], c, sum[4 * j + 2 * h] * ws.x, sum[4 * j + 2 * h + 1] * ws.y, sc, sh);
+                        epi_finish2<MODE, ONE>(P, po[h], c, sum[4 * j + 2 * h] * ws.x, sum[4 * j + 2 * h + 1] * ws.y, sc, sh);
             }
         }
     }
@@ -487,6 +531,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
 // then 8 consecutive words of that strip (hi halves to one plane, lo halves to the other), written 128B-swizzled where
 // wgmma reads it.  Weights (64 x 192 x {hi, lo} = 48 KB) stay resident in shared memory.
 // A tile = 128 consecutive output pixels of one image in raster order (at most two output rows, wo >= 128).
+// ONE (precision "high"): the table's hi half and w_hi only, one wgmma per K=16 step, hi-only store; the lo slots of the
+// shared-memory layout stay unused.
 // Warps: 0 = weight TMA, 4..11 = wgmma consumers (two warpgroups of 64 rows), 12..19 = A-operand producers.
 constexpr int C0T_PROD_WARPS = 8, C0T_STAGES = 3, C0T_K = 192, C0T_ROWS = 8, C0T_STRIDE = 832;
 constexpr int C0T_PSTRIDE = 833;  // words per row of the converted strip: odd, so the 7 filter rows fall into different banks
@@ -494,6 +540,7 @@ constexpr int C0T_PROD0 = 4 + CONS_WARPS;   // first producer warp
 constexpr int C0T_THREADS = (C0T_PROD0 + C0T_PROD_WARPS) * 32;
 constexpr int C0T_SMEM = 1024 + C0T_STAGES * 2 * A_TILE_BYTES + 3 * 2 * 64 * 128 + 2 * C0T_ROWS * C0T_PSTRIDE * 4 + 256 * 4 + 256;
 
+template <bool ONE>
 __global__ void __launch_bounds__(C0T_THREADS, 1)
 k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
            const uint8_t *__restrict__ img, int B, int H, int W, int pad, const float *__restrict__ oscale,
@@ -526,17 +573,17 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
         for (int i = threadIdx.x; i < 256; i += blockDim.x) {
             const float f = (float)i / 255.0f;
             const __half h = __float2half_rn(f), l = __float2half_rn(f - __half2float(h));
-            lut[i] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
+            lut[i] = (uint32_t)__half_as_ushort(h) | (ONE ? 0u : (uint32_t)__half_as_ushort(l) << 16);
         }
     }
     __syncthreads();
 
     if (warp == 0) {
         if (lane == 0) {  // resident weights: three K-slices, hi and lo
-            mbar_expect_tx(wfull_bar, 3 * 2 * 64 * 128);
+            mbar_expect_tx(wfull_bar, (ONE ? 1 : 2) * 3 * 64 * 128);
             for (int s = 0; s < 3; ++s) {
                 tma_3d(smem_base + W_OFF + s * 16384, &tm_w_hi, wfull_bar, s * 64, 0, 0);
-                tma_3d(smem_base + W_OFF + s * 16384 + 8192, &tm_w_lo, wfull_bar, s * 64, 0, 0);
+                if constexpr (!ONE) tma_3d(smem_base + W_OFF + s * 16384 + 8192, &tm_w_lo, wfull_bar, s * 64, 0, 0);
             }
         }
     } else if (warp < 4) {
@@ -556,7 +603,8 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
                 mbar_wait(full_bar(s), (uint32_t)(it / C0T_STAGES) & 1u);
                 const uint32_t sa = smem_base + s * STAGE + wg * 64 * 128, sb = smem_base + W_OFF + ks * 16384;
                 wg_fence();
-                mma_slice<64>(acc, sa, sa + A_TILE_BYTES, sb, sb + 8192, ks == 0);
+                if constexpr (ONE) mma_slice1<64>(acc, sa, sb, ks == 0);
+                else mma_slice<64>(acc, sa, sa + A_TILE_BYTES, sb, sb + 8192, ks == 0);
                 wg_commit();
                 wg_wait<0>();
                 wg_fence_regs(acc);
@@ -579,7 +627,7 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
                     const float2 b2 = __ldg(reinterpret_cast<const float2 *>(shift + c));
                     const float t0 = fmaxf(acc[4 * j + 2 * h] * (w2.x * s2.x) + b2.x, 0.f);
                     const float t1 = fmaxf(acc[4 * j + 2 * h + 1] * (w2.y * s2.y) + b2.y, 0.f);
-                    store_split2(out, oo + c, t0, t1);
+                    store_split2<ONE>(out, oo + c, t0, t1);
                 }
             }
         }
@@ -644,12 +692,13 @@ k_conv0_tc(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ 
                         for (int i = 0; i < 8; ++i) e[i] = src[i];
                         vh = make_uint4(__byte_perm(e[0], e[1], 0x5410), __byte_perm(e[2], e[3], 0x5410),
                                         __byte_perm(e[4], e[5], 0x5410), __byte_perm(e[6], e[7], 0x5410));
-                        vl = make_uint4(__byte_perm(e[0], e[1], 0x7632), __byte_perm(e[2], e[3], 0x7632),
-                                        __byte_perm(e[4], e[5], 0x7632), __byte_perm(e[6], e[7], 0x7632));
+                        if constexpr (!ONE)
+                            vl = make_uint4(__byte_perm(e[0], e[1], 0x7632), __byte_perm(e[2], e[3], 0x7632),
+                                            __byte_perm(e[4], e[5], 0x7632), __byte_perm(e[6], e[7], 0x7632));
                     }
                     const int off = r * 128 + ((j ^ (r & 7)) << 4);       // 128B swizzle: chunk j of row r at (j ^ (r & 7))
                     *reinterpret_cast<uint4 *>(a_hi + off) = vh;
-                    *reinterpret_cast<uint4 *>(a_lo + off) = vl;
+                    if constexpr (!ONE) *reinterpret_cast<uint4 *>(a_lo + off) = vl;
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 __syncwarp();
@@ -716,6 +765,13 @@ static int num_sms() {
 bool tc_plan(const ConvParams &P, TcPlan &plan) {
     plan.ok = false;
     const ConvWeights &w = P.w;
+    // precision "high": weights without a lo plane; every split operand of the layer then has one plane too
+    const bool one = w.lo == nullptr;
+    plan.single = one ? 1 : 0;
+    if (!P.in_scale && (P.a.lo == nullptr) != one) return false;
+    if (P.a2.hi && (P.a2.lo == nullptr) != one) return false;
+    if (P.out_split.hi && (P.out_split.lo == nullptr) != one) return false;
+    if (P.up2 && (P.skip.lo == nullptr) != one) return false;
     if (w.cin_pad % 64 != 0 || w.cout % 32 != 0) return false;
     if (P.stride != 1 && P.stride != 2) return false;
     if (P.pad_t != P.pad_l) return false;
@@ -754,7 +810,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         cuuint32_t box[2] = {64, 128};
         if (!xf) {
             if (!encode(plan.tmap_a_hi, P.a.hi, 2, dims, str, box, ones)) return false;
-            if (!encode(plan.tmap_a_lo, P.a.lo, 2, dims, str, box, ones)) return false;
+            if (!one && !encode(plan.tmap_a_lo, P.a.lo, 2, dims, str, box, ones)) return false;
         } else {
             cuuint64_t rdims[2] = {(cuuint64_t)P.a_raw.c, (cuuint64_t)((long long)P.B * P.a_raw.h * P.a_raw.w)};
             cuuint64_t rstr[1] = {(cuuint64_t)P.a_raw.sW * 4};
@@ -765,7 +821,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
             cuuint64_t d2[2] = {(cuuint64_t)P.a2.c, (cuuint64_t)((long long)P.B * P.a2.h * P.a2.w)};
             cuuint64_t s2[1] = {(cuuint64_t)P.a2.sW * 2};
             if (!encode(plan.tmap_a2_hi, P.a2.hi, 2, d2, s2, box, ones)) return false;
-            if (!encode(plan.tmap_a2_lo, P.a2.lo, 2, d2, s2, box, ones)) return false;
+            if (!one && !encode(plan.tmap_a2_lo, P.a2.lo, 2, d2, s2, box, ones)) return false;
         }
     } else {
         // choose the (bw x bh <= 128) pixel rectangle that wastes the fewest accumulator rows
@@ -788,7 +844,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         cuuint32_t estr[4] = {1, (cuuint32_t)P.stride, (cuuint32_t)P.stride, 1};
         if (!xf) {
             if (!encode(plan.tmap_a_hi, P.a.hi, 4, dims, str, box, estr)) return false;
-            if (!encode(plan.tmap_a_lo, P.a.lo, 4, dims, str, box, estr)) return false;
+            if (!one && !encode(plan.tmap_a_lo, P.a.lo, 4, dims, str, box, estr)) return false;
         } else {
             cuuint64_t rdims[4] = {(cuuint64_t)P.a_raw.c, (cuuint64_t)P.a_raw.w, (cuuint64_t)P.a_raw.h, (cuuint64_t)P.B};
             cuuint64_t rstr[3] = {(cuuint64_t)P.a_raw.sW * 4, (cuuint64_t)P.a_raw.sH * 4, (cuuint64_t)P.a_raw.sN * 4};
@@ -802,7 +858,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
             cuuint32_t box2[4] = {64, (cuuint32_t)(plan.bw * s2), (cuuint32_t)(plan.bh * s2), 1};
             cuuint32_t es2[4] = {1, (cuuint32_t)s2, (cuuint32_t)s2, 1};
             if (!encode(plan.tmap_a2_hi, P.a2.hi, 4, d2, st2, box2, es2)) return false;
-            if (!encode(plan.tmap_a2_lo, P.a2.lo, 4, d2, st2, box2, es2)) return false;
+            if (!one && !encode(plan.tmap_a2_lo, P.a2.lo, 4, d2, st2, box2, es2)) return false;
         }
     }
     {
@@ -810,19 +866,20 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         cuuint64_t str[2] = {(cuuint64_t)w.cin_pad * 2, (cuuint64_t)w.cin_pad * w.cout * 2};
         cuuint32_t box[3] = {64, (cuuint32_t)bn, 1};
         if (!encode(plan.tmap_w_hi, w.hi, 3, dims, str, box, ones)) return false;
-        if (!encode(plan.tmap_w_lo, w.lo, 3, dims, str, box, ones)) return false;
+        if (!one && !encode(plan.tmap_w_lo, w.lo, 3, dims, str, box, ones)) return false;
     }
     plan.ok = true;
     return true;
 }
 
-template <int BLOCK_N, int STAGES, int MODE, bool XF>
+template <int BLOCK_N, int MODE, bool XF, bool ONE>
 static void launch_tm(const ConvParams &P, const TcPlan &plan, const TcGeom &G, cudaStream_t s) {
-    constexpr int smem = tc_smem<BLOCK_N, STAGES, XF>();
+    constexpr int STAGES = tc_stages<BLOCK_N, XF, ONE>();
+    constexpr int smem = tc_smem<BLOCK_N, XF, ONE>(STAGES);
     static_assert(smem <= SMEM_LIMIT, "shared memory budget exceeded");
     static bool attr = false;
     if (!attr) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, MODE, XF>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr = true;
     }
     const int grid = std::min(G.tiles_m * G.tiles_n, num_sms());
@@ -830,23 +887,22 @@ static void launch_tm(const ConvParams &P, const TcPlan &plan, const TcGeom &G, 
     memcpy(&a_hi, plan.tmap_a_hi, 128); memcpy(&a_lo, plan.tmap_a_lo, 128);
     memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
     memcpy(&a2_hi, plan.tmap_a2_hi, 128); memcpy(&a2_lo, plan.tmap_a2_lo, 128);
-    k_conv_tc<BLOCK_N, STAGES, MODE, XF><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
+    k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
 }
 
-// STAGES: as many operand slots as fit 227 KB beside the XF staging ring (BLOCK_N = 128: 64 KB a slot).
-template <int BLOCK_N, int STAGES, int XSTAGES>
+template <int BLOCK_N, bool ONE>
 static void launch_t(const ConvParams &P, const TcPlan &plan, const TcGeom &G, cudaStream_t s) {
     if (P.in_scale) {  // transformed input: only the shapes the plan produces (1x1, plain or upsample epilogue)
         if constexpr (BLOCK_N == 128 || BLOCK_N == 64) {
-            if (P.up2) launch_tm<BLOCK_N, XSTAGES, EPI_UP2, true>(P, plan, G, s);
-            else launch_tm<BLOCK_N, XSTAGES, EPI_PLAIN, true>(P, plan, G, s);
+            if (P.up2) launch_tm<BLOCK_N, EPI_UP2, true, ONE>(P, plan, G, s);
+            else launch_tm<BLOCK_N, EPI_PLAIN, true, ONE>(P, plan, G, s);
             return;
         }
         throw Error(-1, "conv_tc: transformed input with unsupported tile shape");
     }
-    if (P.up2) launch_tm<BLOCK_N, STAGES, EPI_UP2, false>(P, plan, G, s);
-    else if (P.res.p) launch_tm<BLOCK_N, STAGES, EPI_RES, false>(P, plan, G, s);
-    else launch_tm<BLOCK_N, STAGES, EPI_PLAIN, false>(P, plan, G, s);
+    if (P.up2) launch_tm<BLOCK_N, EPI_UP2, false, ONE>(P, plan, G, s);
+    else if (P.res.p) launch_tm<BLOCK_N, EPI_RES, false, ONE>(P, plan, G, s);
+    else launch_tm<BLOCK_N, EPI_PLAIN, false, ONE>(P, plan, G, s);
 }
 
 // Stem launcher.  `w` = conv0 weights as [1 tap][64 cout][192 k] split fp16 (k = ky * 24 + kx * 3 + ch, zeros elsewhere).
@@ -856,24 +912,37 @@ bool conv0_tc_supported(int H, int W, int pad, const SplitRef &out) {
            out.sH % 8 == 0 && out.sN % 8 == 0;
 }
 
+template <bool ONE> static void set_conv0_smem() {
+    static bool attr = false;
+    if (!attr) {
+        HVN_CUDA(cudaFuncSetAttribute(k_conv0_tc<ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C0T_SMEM));
+        attr = true;
+    }
+}
+
 void launch_conv0_tc(const uint8_t *img, int B, int H, int W, int pad, const ConvWeights &w, const float *scale,
                      const float *shift, const SplitRef &out, cudaStream_t s) {
     HVN_CHECK(w.taps == 1 && w.cout == 64 && w.cin_pad == C0T_K, -1, "conv0_tc: unexpected weight layout");
+    const bool one = w.lo == nullptr;
+    HVN_CHECK((out.lo == nullptr) == one, -1, "conv0_tc: weights and output differ in their number of fp16 planes");
     static_assert(C0T_SMEM <= SMEM_LIMIT, "conv0_tc: shared memory budget exceeded");
-    static bool attr = false;
-    if (!attr) {
-        HVN_CUDA(cudaFuncSetAttribute(k_conv0_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, C0T_SMEM));
-        attr = true;
-    }
     alignas(64) CUtensorMap w_hi, w_lo;
     cuuint32_t ones[3] = {1, 1, 1};
     cuuint64_t dims[3] = {(cuuint64_t)w.cin_pad, (cuuint64_t)w.cout, 1};
     cuuint64_t str[2] = {(cuuint64_t)w.cin_pad * 2, (cuuint64_t)w.cin_pad * w.cout * 2};
     cuuint32_t box[3] = {64, 64, 1};
-    HVN_CHECK(encode((unsigned char *)&w_hi, w.hi, 3, dims, str, box, ones) && encode((unsigned char *)&w_lo, w.lo, 3, dims, str, box, ones),
+    memset(&w_lo, 0, sizeof(w_lo));
+    HVN_CHECK(encode((unsigned char *)&w_hi, w.hi, 3, dims, str, box, ones) && (one || encode((unsigned char *)&w_lo, w.lo, 3, dims, str, box, ones)),
               -2, "conv0_tc: tensor map encode failed");
     const int tiles = B * cdiv((long long)out.h * out.w, 128);
-    k_conv0_tc<<<std::min(tiles, num_sms()), C0T_THREADS, C0T_SMEM, s>>>(w_hi, w_lo, img, B, H, W, pad, w.oscale, scale, shift, out);
+    const int grid = std::min(tiles, num_sms());
+    if (one) {
+        set_conv0_smem<true>();
+        k_conv0_tc<true><<<grid, C0T_THREADS, C0T_SMEM, s>>>(w_hi, w_lo, img, B, H, W, pad, w.oscale, scale, shift, out);
+    } else {
+        set_conv0_smem<false>();
+        k_conv0_tc<false><<<grid, C0T_THREADS, C0T_SMEM, s>>>(w_hi, w_lo, img, B, H, W, pad, w.oscale, scale, shift, out);
+    }
 }
 
 void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
@@ -887,10 +956,18 @@ void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
     G.tiles_n = P.w.cout / plan.block_n;
     G.xf_trunc = g_xf_trunc;
     G.pf = g_pf;
-    switch (plan.block_n) {
-    case 128: launch_t<128, 3, 2>(P, plan, G, s); break;
-    case 64: launch_t<64, 4, 3>(P, plan, G, s); break;
-    default: launch_t<32, 5, 2>(P, plan, G, s); break;
+    if (plan.single) {
+        switch (plan.block_n) {
+        case 128: launch_t<128, true>(P, plan, G, s); break;
+        case 64: launch_t<64, true>(P, plan, G, s); break;
+        default: launch_t<32, true>(P, plan, G, s); break;
+        }
+    } else {
+        switch (plan.block_n) {
+        case 128: launch_t<128, false>(P, plan, G, s); break;
+        case 64: launch_t<64, false>(P, plan, G, s); break;
+        default: launch_t<32, false>(P, plan, G, s); break;
+        }
     }
 }
 

@@ -18,10 +18,14 @@ def convert_pytorch_checkpoint(net_state_dict):
 
 
 class HoVerNet(object):
-    def __init__(self, input_ch=3, nr_types=None, freeze=False, mode="original", device=None):
+    """precision: "highest" (default) or "high" -- see `_lib.Context`.  An extension: the reference has no such
+    argument (its PyTorch convolutions run in TF32 on this GPU by default)."""
+
+    def __init__(self, input_ch=3, nr_types=None, freeze=False, mode="original", device=None, precision="highest"):
         assert mode == "original" or mode == "fast", \
             "Unknown mode `%s` for HoVerNet %s. Only support `original` or `fast`." % (mode, "")
         assert input_ch == 3, "only RGB input is supported"
+        _lib.precision_code(precision)  # ValueError before a context exists
         self.mode = mode
         self.freeze = freeze
         self.nr_types = nr_types
@@ -30,7 +34,8 @@ class HoVerNet(object):
         if device is None:
             import os
             device = int(os.environ.get("LOCAL_RANK", "0"))
-        self.ctx = _lib.Context(device, mode, nr_types)
+        self.precision = precision
+        self.ctx = _lib.Context(device, mode, nr_types, precision=precision)
         self._loaded = False
 
     # ---- torch.nn.Module look-alikes used by reference infer/base.py:64-70
@@ -70,7 +75,7 @@ class HoVerNet(object):
         raise RuntimeError("call models.hovernet.run_desc.infer_step(batch, model) -- the fused device path")
 
 
-def create_model(mode=None, **kwargs):
+def create_model(mode=None, *, precision="highest", **kwargs):
     if mode not in ["original", "fast"]:
         assert "Unknown Model Mode %s" % mode
-    return HoVerNet(mode=mode, **kwargs)
+    return HoVerNet(mode=mode, precision=precision, **kwargs)

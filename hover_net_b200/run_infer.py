@@ -9,6 +9,12 @@ Same option names, defaults and `method_args` / `run_args` dictionaries as refer
 one process drives one GPU (`--gpu` takes the first id of the list unless the process was launched by
 torchrun, where LOCAL_RANK picks the device and files / patches are sharded over the ranks), and
 `--nr_inference_workers` / `--nr_post_proc_workers` are accepted and ignored (no CPU stage is left).
+
+Extension the reference CLI lacks: `--precision {highest,high}` (default `highest`) picks the convolution operand
+precision.  `highest` forms fp32-grade products (fp16 hi + lo operands); `high` stores every activation and weight
+that feeds a convolution as one fp16 value and forms one product per multiply-accumulate, with fp32 accumulation --
+the operand precision the reference itself gets from PyTorch's default TF32 convolutions on this GPU -- for a third of
+the tensor-core work.  A non-default value is passed to `create_model` through `method_args["method"]["model_args"]`.
 """
 import argparse
 import logging
@@ -29,6 +35,7 @@ def _top_parser():
     ap.add_argument("--nr_inference_workers", default="8")
     ap.add_argument("--nr_post_proc_workers", default="16")
     ap.add_argument("--batch_size", default="32")
+    ap.add_argument("--precision", default="highest", choices=["highest", "high"])
     return ap
 
 
@@ -79,6 +86,8 @@ def parse(argv, nr_gpus=1):
         },
         "type_info_path": None if args.type_info_path == "" else args.type_info_path,
     }
+    if args.precision != "highest":  # the default leaves model_args exactly as the reference builds them
+        method_args["method"]["model_args"]["precision"] = args.precision
     run_args = {
         "batch_size": int(args.batch_size) * max(1, nr_gpus),
         "nr_inference_workers": int(args.nr_inference_workers),

@@ -74,6 +74,14 @@ int hvn_finalize_weights(hvn_ctx *ctx);
  *                      "chunk" = patches per internal sub-batch (0 = auto);
  *                      "act_shift" = s in 0..48: store activations as x * 2^-s (see HVN_ERR_RANGE; weights are
  *                      re-derived, results are unchanged because powers of two are exact);
+ *                      "precision" = 0 "highest" (default): activations feeding a convolution and its weights are
+ *                      stored as fp16 hi + lo and each MAC forms hi*hi + hi*lo + lo*hi (fp32-grade products);
+ *                      1 "high": hi planes only, one fp16 product per MAC with fp32 accumulation -- the operand
+ *                      precision of TF32, a third of the tensor-core work and about half the activation memory.
+ *                      Residual sums, BatchNorm, the 1x1 heads and post-processing stay fp32 in both; the range rules
+ *                      (HVN_ERR_RANGE, "act_shift") are the same.  A change synchronises the context, re-derives the
+ *                      weights and drops the cached plans; setting 0 again reproduces "highest" bit for bit.
+ *                      Any other value is HVN_ERR_INVALID;
  *                      "profile" = 0 | 1 | 2 (see hvn_stage_ms);
  *                      tuning knobs: "tc_seg_chunks" (64-channel slices per accumulation segment), "tc_block_n",
  *                      "tc_prefetch" (L2 prefetch distance in K-slices for flat operands, 0 = off), "tc_xf_trunc"
@@ -84,7 +92,8 @@ int hvn_finalize_weights(hvn_ctx *ctx);
 int hvn_set_option(hvn_ctx *ctx, const char *key, int64_t value);
 const char *hvn_debug_log(const hvn_ctx *ctx);
 /* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing and contour kernels), "last_flops" (algorithmic 2*MACs of the
- * last forward); with option "profile" = 2 also "launches:<class>" and "flops:<class>" for
+ * last forward), "precision" (0 | 1), "plan_bytes" (device bytes of the activation buffers of the plan(s) the last
+ * forward ran); with option "profile" = 2 also "launches:<class>" and "flops:<class>" for
  * class in {conv_tc, conv_ref, conv0, bnrelu, head} (see hvn_stage_ms). */
 int64_t hvn_get_counter(const hvn_ctx *ctx, const char *key);
 
