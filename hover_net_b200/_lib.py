@@ -8,6 +8,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libhvn.so")
 ROW_LEN = 10
+# hvn_targets flag bits (include/hvn.h HVN_TG_*): the maps the reference's gen_instance_hv_map raises ValueError on
+TG_NO_BACKGROUND, TG_NO_BACKGROUND_CROP, TG_EMPTY_BOX = 1, 2, 4
 _lib = None
 
 
@@ -268,6 +270,58 @@ class Context:
             return False
         check(rc)
         return True
+
+    _TARGETS_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+
+    def targets(self, inst, crop_shape):
+        """Full-size HV targets of instance maps inst [H,W] or [n,H,W] (the reference's gen_instance_hv_map):
+        returns (hv float32 [n,H,W,2] (x, y), flags int32 [n] -- TG_* bits, the maps the reference rejects)."""
+        a = _as_ids(inst)
+        if a.ndim == 2:
+            a = a[None]
+        n, H, W = a.shape
+        hv = np.empty((n, H, W, 2), dtype=np.float32)
+        flags = np.zeros((n,), dtype=np.int32)
+        L = lib()
+        L.hvn_targets.argtypes = self._TARGETS_ARGS
+        check(L.hvn_targets(self._h, _ptr(a), n, H, W, int(crop_shape[0]), int(crop_shape[1]), _ptr(hv), _ptr(flags)))
+        return hv, flags
+
+    def targets_dev(self, d_inst, n, H, W, crop_h, crop_w, d_hv, d_flags):
+        L = lib()
+        L.hvn_targets_dev.argtypes = self._TARGETS_ARGS
+        check(L.hvn_targets_dev(self._h, _ptr(d_inst), int(n), int(H), int(W), int(crop_h), int(crop_w), _ptr(d_hv),
+                                _ptr(d_flags)))
+
+    _VALID_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                   ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+
+    def valid(self, imgs_u8, inst, type_map=None):
+        """One validation batch through forward, targets and counts on the device (model contexts).  imgs uint8
+        [B,H,W,3], inst / type_map int32 [B,H,W] at the network input size.  Returns (counts int64 [3 + 2*nr_types]
+        = correct, inter, total, then inter_k, total_k per type; hv_sse float; flags int32 [B])."""
+        x = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
+        B, H, W, C = x.shape
+        assert C == 3
+        a = _as_ids(inst)
+        t = None if type_map is None or not self.nr_types else _as_ids(type_map)
+        if a.shape != (B, H, W) or (t is not None and t.shape != (B, H, W)):
+            raise ValueError("inst / type maps must be [B,H,W] = %s" % ((B, H, W),))
+        counts = np.zeros((3 + 2 * int(self.nr_types or 0),), dtype=np.int64)
+        sse = np.zeros((1,), dtype=np.float64)
+        flags = np.zeros((B,), dtype=np.int32)
+        L = lib()
+        L.hvn_valid.argtypes = self._VALID_ARGS
+        check(self._retry_range(lambda: L.hvn_valid(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
+                                                    _ptr(sse), _ptr(flags))))
+        return counts, float(sse[0]), flags
+
+    def valid_dev(self, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags):
+        L = lib()
+        L.hvn_valid_dev.argtypes = self._VALID_ARGS
+        check(L.hvn_valid_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
+                              _ptr(d_counts), _ptr(d_sse), _ptr(d_flags)))
 
     def tile_grid(self, H, W, patch_in):
         r, c = ctypes.c_int(), ctypes.c_int()

@@ -19,6 +19,7 @@ SOURCES = [
     ("contour.cu", []),
     ("tile.cu", []),
     ("stats.cu", []),
+    ("targets.cu", []),
 ]
 
 

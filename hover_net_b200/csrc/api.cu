@@ -2,11 +2,13 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <vector>
 
 #include "../../include/hvn.h"
 #include "cnn.h"
 #include "postproc.h"
 #include "stats.h"
+#include "targets.h"
 #include "tile.h"
 
 using namespace hvn;
@@ -21,6 +23,8 @@ struct hvn_ctx {
     Arena io_arena;                // staging for the host-pointer entry points
     Arena tile_arena;              // patch / output batches of the tile path
     Arena stats_arena;             // pair-table workspace of hvn_inst_pairs*
+    Arena targets_arena;           // workspace of hvn_targets* and hvn_valid*
+    Arena valid_arena;             // maps and counts of hvn_valid*
     int chunk = 0;
     int profile = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -92,6 +96,8 @@ void hvn_destroy(hvn_ctx *c) {
     c->io_arena.release();
     c->tile_arena.release();
     c->stats_arena.release();
+    c->targets_arena.release();
+    c->valid_arena.release();
     for (auto &e : c->ev) cudaEventDestroy(e);
     for (auto &e : c->tev) cudaEventDestroy(e);
     cudaStreamDestroy(c->stream);
@@ -539,6 +545,127 @@ int hvn_inst_pairs(hvn_ctx *c, const int32_t *tru, const int32_t *pred, int n, i
     inst_pairs_emit(c->stream, w, d_pairs, total);
     HVN_CUDA(cudaMemcpyAsync(pairs, d_pairs, (size_t)total * 24, cudaMemcpyDeviceToHost, c->stream));
     HVN_CUDA(cudaStreamSynchronize(c->stream));
+    API_END
+}
+
+// ---------------------------------------------------------------------------------------------------
+static void check_targets_args(int n, int H, int W, int crop_h, int crop_w) {
+    HVN_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1, HVN_ERR_INVALID, "bad shape");
+    HVN_CHECK((long long)H * W <= 0x7fffffffll, HVN_ERR_INVALID, "map larger than 2^31 - 1 pixels");
+    HVN_CHECK(crop_h >= 1 && crop_h <= H && crop_w >= 1 && crop_w <= W, HVN_ERR_INVALID,
+              "crop shape must lie within the map");
+}
+// After the context stream has been synchronised.
+static void check_targets_result(const TargetWork &w) {
+    std::vector<int> per((size_t)5 * w.n + 1);
+    HVN_CUDA(cudaMemcpy(per.data(), w.maxid, per.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    HVN_CHECK(!per[(size_t)5 * w.n], HVN_ERR_INVALID, "negative instance id");
+    for (int m = 0; m < w.n; ++m)
+        HVN_CHECK((long long)per[m] + per[(size_t)w.n + m] <= 0x7fffffffll, HVN_ERR_INVALID,
+                  "map " + std::to_string(m) + ": largest id " + std::to_string(per[m]) + " + " +
+                      std::to_string(per[(size_t)w.n + m]) +
+                      " components exceeds 2^31 - 1 (the fresh ids of split instances would not fit in int32)");
+}
+
+int hvn_targets_dev(hvn_ctx *c, const int32_t *inst, int n, int H, int W, int crop_h, int crop_w, float *hv,
+                    int32_t *flags) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(inst && hv && flags, HVN_ERR_INVALID, "null buffer");
+    check_targets_args(n, H, W, crop_h, crop_w);
+    TargetWork w;
+    targets_run(c->targets_arena, c->stream, inst, n, H, W, crop_h, crop_w, hv, flags, w);
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    check_targets_result(w);
+    API_END
+}
+
+int hvn_targets(hvn_ctx *c, const int32_t *inst, int n, int H, int W, int crop_h, int crop_w, float *hv,
+                int32_t *flags) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(inst && hv && flags, HVN_ERR_INVALID, "null buffer");
+    check_targets_args(n, H, W, crop_h, crop_w);
+    const size_t px = (size_t)n * H * W;
+    c->io_arena.reset();
+    c->io_arena.reserve(px * 12 + (size_t)n * 4 + 4096);
+    int32_t *d_inst = c->io_arena.take<int32_t>(px);
+    float *d_hv = c->io_arena.take<float>(px * 2);
+    int32_t *d_flags = c->io_arena.take<int32_t>(n);
+    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
+    TargetWork w;
+    targets_run(c->targets_arena, c->stream, d_inst, n, H, W, crop_h, crop_w, d_hv, d_flags, w);
+    HVN_CUDA(cudaMemcpyAsync(hv, d_hv, px * 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    check_targets_result(w);
+    API_END
+}
+
+// Forward, targets and counts of one batch, enqueued on the context stream; the caller synchronises and checks.
+static void run_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                      int64_t *counts, double *sse, int32_t *flags, TargetWork &w) {
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    const int nt = c->model->nr_types;
+    HVN_CHECK(imgs && inst && counts && sse && flags, HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(nt == 0 || type, HVN_ERR_INVALID, "a model with nr_types > 0 needs a type map");
+    int oh, ow, oc;
+    c->model->out_shape(H, W, oh, ow, oc);
+    check_targets_args(B, H, W, oh, ow);
+    const size_t opx = (size_t)B * oh * ow, px = (size_t)B * H * W;
+    c->valid_arena.reset();
+    c->valid_arena.reserve(opx * oc * 4 + px * 8 + 1024);
+    float *d_pred = c->valid_arena.take<float>(opx * oc);
+    float *d_hv = c->valid_arena.take<float>(px * 2);
+    HVN_CUDA(cudaMemsetAsync(counts, 0, (size_t)(3 + 2 * nt) * 8, c->stream));
+    HVN_CUDA(cudaMemsetAsync(sse, 0, sizeof(double), c->stream));
+    run_forward(c, imgs, B, H, W, d_pred);
+    targets_run(c->targets_arena, c->stream, inst, B, H, W, oh, ow, d_hv, flags, w);
+    valid_reduce(c->stream, d_pred, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, oc, nt, (long long *)counts, sse);
+}
+
+int hvn_valid_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                  int64_t *counts, double *sse, int32_t *flags) {
+    API_BEGIN
+    use(c);
+    TargetWork w;
+    run_valid(c, imgs, inst, type, B, H, W, counts, sse, flags, w);
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    finish_profile(c, true, false);
+    check_range(c);
+    check_targets_result(w);
+    API_END
+}
+
+int hvn_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+              int64_t *counts, double *sse, int32_t *flags) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    HVN_CHECK(imgs && inst && counts && sse && flags, HVN_ERR_INVALID, "null buffer");
+    check_targets_args(B, H, W, 1, 1);
+    const int nt = c->model->nr_types;
+    const size_t px = (size_t)B * H * W, nc = 3 + 2 * (size_t)nt;
+    c->io_arena.reset();
+    c->io_arena.reserve(px * 3 + px * 4 * (nt ? 2 : 1) + nc * 8 + (size_t)B * 4 + 8 + 4096);
+    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
+    int32_t *d_inst = c->io_arena.take<int32_t>(px);
+    int32_t *d_type = nt && type ? c->io_arena.take<int32_t>(px) : nullptr;
+    int64_t *d_counts = c->io_arena.take<int64_t>(nc);
+    double *d_sse = c->io_arena.take<double>(1);
+    int32_t *d_flags = c->io_arena.take<int32_t>(B);
+    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
+    if (d_type) HVN_CUDA(cudaMemcpyAsync(d_type, type, px * 4, cudaMemcpyHostToDevice, c->stream));
+    TargetWork w;
+    run_valid(c, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags, w);
+    HVN_CUDA(cudaMemcpyAsync(counts, d_counts, nc * 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(sse, d_sse, 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    finish_profile(c, true, false);
+    check_range(c);
+    check_targets_result(w);
     API_END
 }
 

@@ -19,6 +19,7 @@
 //   :120-181 per-instance bbox/centroid/type   k_table_accum k_table_rows
 #include "common.cuh"
 #include "postproc.h"
+#include "uf.cuh"
 
 #include <string>
 #include <utility>
@@ -111,27 +112,8 @@ __global__ void k_threshold_minmax(const float *__restrict__ pred, int C, int of
 }
 
 // ------------------------------------------------------------------------------------------------
-// 4-connected component labelling by union-find; root = smallest linear index of the component,
+// 4-connected component labelling by union-find (uf.cuh); root = smallest linear index of the component,
 // i.e. the component's first pixel in raster order (what scipy.ndimage.label numbers by).
-__device__ __forceinline__ int uf_find(const int *L, int a) {
-    int r = a;
-    while (true) {
-        int p = L[r];
-        if (p == r) return r;
-        r = p;
-    }
-}
-__device__ __forceinline__ void uf_union(int *L, int a, int b) {
-    while (true) {
-        a = uf_find(L, a);
-        b = uf_find(L, b);
-        if (a == b) return;
-        if (a > b) { int t = a; a = b; b = t; }
-        int old = atomicMin(&L[b], a);  // hang the larger root under the smaller one
-        if (old == b) return;
-        b = old;
-    }
-}
 
 // inv = 0: label pixels where src != 0 ; inv = 1: label pixels where src == 0 (for hole filling)
 __global__ void k_ccl_init(const unsigned char *__restrict__ src, int inv, int N, int *__restrict__ L) {

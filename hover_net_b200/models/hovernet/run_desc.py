@@ -1,4 +1,5 @@
-"""Drop-in for reference `models/hovernet/run_desc.py:171-197` (`infer_step`)."""
+"""Drop-in for reference `models/hovernet/run_desc.py`: `infer_step` (:171-197), `valid_step` (:113-167) and
+`proc_valid_step_output` (:263-344, scalars only)."""
 import numpy as np
 
 
@@ -26,3 +27,71 @@ def infer_step_fused(batch_data, model, return_pred=True):
     Returns (pred or None, inst [B,h,w] int32, table [B,max_rows,10] int64, n_rows [B])."""
     net = getattr(model, "module", model)
     return net.ctx.forward_postproc(_as_u8(batch_data), want_pred=return_pred)
+
+
+def _host(x):
+    return x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
+
+
+def valid_step(batch_data, run_info):
+    """Reference `valid_step`: batch_data {"img" [B,H,W,3], "np_map" [B,h,w], "hv_map" [B,h,w,2], "tp_map"
+    [B,h,w] with types}, run_info = (run_info, state_info) with run_info["net"]["desc"] the model.  Returns the
+    reference's {"raw": {"imgs", "true_np", "true_hv", "prob_np", "pred_hv", ["true_tp", "pred_tp"]}}.  Unlike the
+    reference, a batch of one patch keeps its batch axis (the reference's squeeze drops it)."""
+    run_info, _state_info = run_info
+    net = getattr(run_info["net"]["desc"], "module", run_info["net"]["desc"])
+    imgs = _as_u8(batch_data["img"])
+    pred = net.ctx.forward(imgs)
+    raw = {
+        "imgs": _host(batch_data["img"]),
+        "true_np": _host(batch_data["np_map"]).astype(np.int64),
+        "true_hv": _host(batch_data["hv_map"]).astype(np.float32),
+        "prob_np": np.ascontiguousarray(pred[..., -3]),
+        "pred_hv": np.ascontiguousarray(pred[..., -2:]),
+    }
+    if net.nr_types is not None:
+        raw["true_tp"] = _host(batch_data["tp_map"]).astype(np.int64)
+        raw["pred_tp"] = np.ascontiguousarray(pred[..., 0])
+    return {"raw": raw}
+
+
+def valid_scalars(correct, inter, total, type_counts, hv_sse, nr_pixels):
+    """The reference's scalars from integer counts: np_acc, np_dice, tp_dice_<k> (type_counts: [(inter_k,
+    total_k)] or None), hv_mse.  The integer ratios are evaluated exactly as the reference evaluates them."""
+    out = {}
+    out["np_acc"] = np.int64(correct) / nr_pixels
+    out["np_dice"] = 2 * np.int64(inter) / (np.int64(total) + 1.0e-8)
+    for k, (ik, tk) in enumerate(type_counts or ()):
+        out["tp_dice_%d" % k] = 2 * np.int64(ik) / (np.int64(tk) + 1.0e-8)
+    out["hv_mse"] = hv_sse / nr_pixels
+    return out
+
+
+def proc_valid_step_output(raw_data, nr_types=None):
+    """Reference `proc_valid_step_output`, restated on host numpy arrays with the same operations on the same
+    values, so the scalars are bit-identical.  Returns {"scalar": {...}, "image": {}}: the reference's image entry
+    is a matplotlib figure, and matplotlib is not a dependency of this package."""
+    prob_np, true_np = raw_data["prob_np"], raw_data["true_np"]
+    n = len(true_np)
+    pred_np = (np.asarray(prob_np) > 0.5).astype(np.int32)
+    true_np = np.asarray(true_np)
+    correct = int((pred_np == true_np).sum())
+    t1 = (true_np == 1).astype(np.int32)
+    p1 = (pred_np == 1).astype(np.int32)
+    inter, total = int((t1 * p1).sum()), int((t1 + p1).sum())
+    type_counts = None
+    if nr_types is not None:
+        pred_tp, true_tp = np.asarray(raw_data["pred_tp"]), np.asarray(raw_data["true_tp"])
+        type_counts = []
+        for k in range(nr_types):
+            tk = (true_tp == k).astype(np.int32)
+            pk = (pred_tp == k).astype(np.int32)
+            type_counts.append((int((tk * pk).sum()), int((tk + pk).sum())))
+    # float32 per-patch sums accumulated in patch order, as the reference does
+    sse = 0
+    for i in range(n):
+        d = raw_data["pred_hv"][i] - raw_data["true_hv"][i]
+        sse += (d * d).sum()
+    nr_pixels = n * np.size(true_np[0])
+    scalar = valid_scalars(correct, inter, total, type_counts, sse, nr_pixels)
+    return {"scalar": scalar, "image": {}}

@@ -176,6 +176,35 @@ int hvn_inst_pairs(hvn_ctx *ctx, const int32_t *true_host, const int32_t *pred_h
 int hvn_inst_pairs_dev(hvn_ctx *ctx, const int32_t *true_dev, const int32_t *pred_dev, int n_maps, int H, int W,
                        int64_t *pairs_dev, int64_t cap, int64_t *offs_dev);
 
+/* ---- training targets (reference models/hovernet/targets.py gen_instance_hv_map, including
+ * dataloader/augs.py fix_mirror_padding): inst int32 [n_maps,H,W] (ids >= 0, 0 = background) -> hv float32
+ * [n_maps,H,W,2] (x, y), the full-size map before gen_targets crops it to crop_h x crop_w (the crop decides which
+ * instances get offsets: those with >= 30 pixels inside it), bit for bit.  flags int32 [n_maps], HVN_TG_* bits: the
+ * cases in which the reference raises ValueError (hv is undefined for such a map).  HVN_ERR_INVALID on a negative
+ * id, on crop_h/crop_w outside 1..H/1..W, and when a map's largest id + its number of 4-connected components exceeds
+ * 2^31 - 1 (the reference's int32 renumbering of split instances would wrap).  n_maps <= 65535, H*W < 2^31.  Device
+ * workspace (context-owned, grow-only): 60 B per pixel.  Both variants synchronise the context stream. */
+#define HVN_TG_NO_BACKGROUND 1       /* no 0 pixel in the map */
+#define HVN_TG_NO_BACKGROUND_CROP 2  /* no 0 pixel left in the crop after removing instances < 30 px there */
+#define HVN_TG_EMPTY_BOX 4           /* an instance's wrapped box holds none of its pixels (NaN centre of mass) */
+int hvn_targets(hvn_ctx *ctx, const int32_t *inst_host, int n_maps, int H, int W, int crop_h, int crop_w,
+                float *hv_host, int32_t *flags_host);
+int hvn_targets_dev(hvn_ctx *ctx, const int32_t *inst_dev, int n_maps, int H, int W, int crop_h, int crop_w,
+                    float *hv_dev, int32_t *flags_dev);
+
+/* ---- validation step (reference run_desc.py valid_step + proc_valid_step_output) on one batch of patches already
+ * cropped to the network input: imgs u8 [B,H,W,3], inst int32 [B,H,W], type int32 [B,H,W] (required when the model
+ * has nr_types > 0, ignored otherwise).  Runs the forward (honouring "precision", "act_shift" and HVN_ERR_RANGE like
+ * every forward), the targets on the same stream, and one reduction over the hvn_out_shape centre crop:
+ * counts int64 [3 + 2*nr_types] = correct, inter, total of (np_prob > 0.5) against (inst > 0), then inter_k,
+ * total_k of (tp == k) against (type == k) for k = 0..nr_types-1; hv_sse = sum of (pred_hv - true_hv)^2 (fp32
+ * differences, fp64 sum); flags [B] as for hvn_targets.  Outputs are overwritten, not accumulated.  The maps never
+ * leave the device.  Both variants synchronise the context stream. */
+int hvn_valid(hvn_ctx *ctx, const uint8_t *imgs_host, const int32_t *inst_host, const int32_t *type_host, int B, int H,
+              int W, int64_t *counts_host, double *hv_sse_host, int32_t *flags_host);
+int hvn_valid_dev(hvn_ctx *ctx, const uint8_t *imgs_dev, const int32_t *inst_dev, const int32_t *type_dev, int B,
+                  int H, int W, int64_t *counts_dev, double *hv_sse_dev, int32_t *flags_dev);
+
 /* ---- device memory / stream helpers for callers without a CUDA binding of their own. */
 int hvn_malloc(hvn_ctx *ctx, size_t bytes, void **dev_ptr);
 int hvn_free(hvn_ctx *ctx, void *dev_ptr);
