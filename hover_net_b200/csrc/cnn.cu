@@ -222,11 +222,20 @@ void Model::make_conv_concat(const std::string &key, const std::string &name1, c
     conv_[key] = cw;
 }
 
+// BatchNorm and head parameters must be finite: the reference would return NaN maps for them, which the engine's ReLU
+// and range clamp would otherwise turn into finite, plausible-looking ones
+static void check_finite(const std::vector<float> &v, const std::string &name) {
+    for (float x : v) HVN_CHECK(std::isfinite(x), -3, "non-finite value in checkpoint parameter " + name);
+}
+
 // eval-mode BatchNorm2d(eps=1e-5) as y = x*scale + shift
 void Model::make_bn(const std::string &p) {
     const auto &g = hostp(p + ".weight"), &b = hostp(p + ".bias"), &m = hostp(p + ".running_mean"),
                &v = hostp(p + ".running_var");
+    for (const char *f : {".weight", ".bias", ".running_mean", ".running_var"}) check_finite(hostp(p + f), p + f);
     int c = (int)g.size();
+    for (int i = 0; i < c; ++i)
+        HVN_CHECK((double)v[i] + 1e-5 > 0.0, -3, "running_var + eps <= 0 in checkpoint parameter " + p + ".running_var");
     std::vector<float> sc(c), sh(c);
     for (int i = 0; i < c; ++i) {
         double s = (double)g[i] / std::sqrt((double)v[i] + 1e-5);
@@ -318,12 +327,14 @@ void Model::finalize() {
             }
         } else if (n.size() > 15 && n.compare(n.size() - 15, 15, ".u0.conv.weight") == 0) {
             std::vector<float> w = hostp(n);
+            check_finite(w, n);
             for (auto &x : w) x = std::ldexp(x, act_shift);  // the heads see features scaled by 2^-act_shift
             float *d = dalloc<float>(w.size(), wallocs_, false);
             HVN_CUDA(cudaMemcpy(d, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
             head_w_[n.substr(0, n.size() - 7)] = d;
         } else if (n.size() > 13 && n.compare(n.size() - 13, 13, ".u0.conv.bias") == 0) {
             const auto &w = hostp(n);
+            check_finite(w, n);
             float *d = dalloc<float>(w.size(), wallocs_, false);
             HVN_CUDA(cudaMemcpy(d, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
             head_b_[n.substr(0, n.size() - 5)] = d;

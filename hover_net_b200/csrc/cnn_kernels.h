@@ -50,5 +50,7 @@ void tc_set_block_n(int n);      // tuning knobs (0 = automatic)
 void tc_set_seg_chunks(int n);
 void tc_set_prefetch(int n);     // L2 prefetch distance in K-slices for flat (2-D map) operands, 0 = off
 void tc_set_xf_trunc(int on);    // XF transform warps: truncating hi/lo split (1, default) or round-to-nearest (0)
+// the k_conv_tc instantiation the last tc_launch issued: BLOCK_N | epilogue (EPI_*) << 8 | XF << 12 | ONE << 13
+int tc_last_dispatch();
 
 }  // namespace hvn

@@ -6,8 +6,10 @@
 
 namespace hvn {
 
+// The range tests are written !(|x| <= 65504) so that NaN, for which every comparison is false, raises the flag too; the
+// clamp then stores it as -65504 (fmaxf returns the non-NaN operand), finite like every other flagged value.
 __device__ __forceinline__ void split_f32(float x, __half &hi, __half &lo, unsigned int *flag = nullptr) {
-    if (flag && fabsf(x) > 65504.f) *flag = 1u;  // benign race: every writer stores the same value
+    if (flag && !(fabsf(x) <= 65504.f)) *flag = 1u;  // benign race: every writer stores the same value
     x = fminf(fmaxf(x, -65504.f), 65504.f);
     hi = __float2half_rn(x);
     lo = __float2half_rn(x - __half2float(hi));
@@ -18,8 +20,16 @@ __device__ __forceinline__ float join_f16(__half hi, __half lo) { return __half2
 // Single-plane tensors (precision "high": SplitRef::lo == nullptr) store only hi = fp16_rn(x) -- the same hi, with the same
 // range check and clamp, as split_f32 -- and read back as hi alone.
 __device__ __forceinline__ __half hi_f32(float x, unsigned int *flag = nullptr) {
-    if (flag && fabsf(x) > 65504.f) *flag = 1u;
+    if (flag && !(fabsf(x) <= 65504.f)) *flag = 1u;
     return __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
+}
+
+// max that returns NaN when either operand is NaN (fmaxf returns the other one): a running maximum built from it carries
+// a NaN through to the range test
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
 }
 
 // Four values at once with the packed conversions (one F2FP per pair): same roundings as split_f32.
@@ -27,9 +37,9 @@ __device__ __forceinline__ __half hi_f32(float x, unsigned int *flag = nullptr) 
 template <bool NONNEG = false>
 __device__ __forceinline__ void split4_f32(const float t[4], uint2 &hi, uint2 &lo, unsigned int *flag = nullptr) {
     if (flag) {
-        const float m = NONNEG ? fmaxf(fmaxf(t[0], t[1]), fmaxf(t[2], t[3]))
-                               : fmaxf(fmaxf(fabsf(t[0]), fabsf(t[1])), fmaxf(fabsf(t[2]), fabsf(t[3])));
-        if (m > 65504.f) *flag = 1u;
+        const float m = NONNEG ? fmax_nan(fmax_nan(t[0], t[1]), fmax_nan(t[2], t[3]))
+                               : fmax_nan(fmax_nan(fabsf(t[0]), fabsf(t[1])), fmax_nan(fabsf(t[2]), fabsf(t[3])));
+        if (!(m <= 65504.f)) *flag = 1u;
     }
     float x[4];
 #pragma unroll

@@ -250,8 +250,12 @@ __global__ void __launch_bounds__(256) k_bnrelu(RawRef in, int B, const float *_
                                                            (long long)x * in.sW + c);
         const float4 s = *reinterpret_cast<const float4 *>(scale + c);
         const float4 b = *reinterpret_cast<const float4 *>(shift + c);
-        float tt[4] = {fmaxf(v.x * s.x + b.x, 0.f), fmaxf(v.y * s.y + b.y, 0.f), fmaxf(v.z * s.z + b.z, 0.f),
-                       fmaxf(v.w * s.w + b.w, 0.f)};
+        float tt[4] = {v.x * s.x + b.x, v.y * s.y + b.y, v.z * s.z + b.z, v.w * s.w + b.w};
+        // a NaN input raises the range flag like it does in the XF transform that replaces this pass (the ReLU below
+        // would turn it into 0)
+        if (out.flag && (tt[0] != tt[0] || tt[1] != tt[1] || tt[2] != tt[2] || tt[3] != tt[3])) *out.flag = 1u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tt[k] = fmaxf(tt[k], 0.f);
         __half oh[4], ol[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) split_f32(tt[k], oh[k], ol[k], out.flag);

@@ -395,14 +395,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 mbar_wait(empty_bar(s), ph ^ 1u);
                 uint8_t *a_hi = smem_gen + s * STAGE_BYTES, *a_lo = a_hi + A_TILE_BYTES;
                 // range guard: running maximum, tested once per tile (a flag store inside this loop cost the XF layers
-                // 40-60 %, measured).  128B swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7)).
+                // 40-60 %, measured).  It is taken before the ReLU with a NaN-propagating max (starting from 0, the same
+                // maximum for finite values), so a NaN in the raw input raises the flag too.  128B swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7)).
                 if constexpr (ONE) {  // hi = fp16_rn(relu(y)): round to nearest -- truncation is only valid with a lo plane
 #pragma unroll
                     for (int i = 0; i < XR; ++i) {
                         const int row = rg + RG * i;
                         if (128 % RG != 0 && i == XR - 1 && row >= 128) break;
                         const float y4[4] = {fmaxf(v[i].x, 0.f), fmaxf(v[i].y, 0.f), fmaxf(v[i].z, 0.f), fmaxf(v[i].w, 0.f)};
-                        rmax = fmaxf(fmaxf(rmax, fmaxf(y4[0], y4[1])), fmaxf(y4[2], y4[3]));
+                        rmax = fmax_nan(fmax_nan(rmax, fmax_nan(v[i].x, v[i].y)), fmax_nan(v[i].z, v[i].w));
                         const int off = row * 128 + ((((l16 >> 1) ^ (row & 7))) << 4) + (l16 & 1) * 8;
                         *reinterpret_cast<uint2 *>(a_hi + off) = hi4_f32_nonneg(y4);
                     }
@@ -413,7 +414,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                         if (128 % RG != 0 && i == XR - 1 && row >= 128) break;
                         const float y4[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
                         uint2 oh, ol;
-                        rmax = fmaxf(fmaxf(rmax, fmaxf(y4[0], y4[1])), fmaxf(y4[2], y4[3]));
+                        rmax = fmax_nan(fmax_nan(rmax, fmax_nan(y4[0], y4[1])), fmax_nan(y4[2], y4[3]));
                         split4_relu_trunc(y4, oh, ol);
                         const int off = row * 128 + ((((l16 >> 1) ^ (row & 7))) << 4) + (l16 & 1) * 8;
                         *reinterpret_cast<uint2 *>(a_hi + off) = oh;
@@ -426,7 +427,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                         if (128 % RG != 0 && i == XR - 1 && row >= 128) break;
                         float y4[4] = {fmaxf(v[i].x, 0.f), fmaxf(v[i].y, 0.f), fmaxf(v[i].z, 0.f), fmaxf(v[i].w, 0.f)};
                         uint2 oh, ol;
-                        rmax = fmaxf(fmaxf(rmax, fmaxf(y4[0], y4[1])), fmaxf(y4[2], y4[3]));
+                        rmax = fmax_nan(fmax_nan(rmax, fmax_nan(v[i].x, v[i].y)), fmax_nan(v[i].z, v[i].w));
                         split4_f32<true>(y4, oh, ol);
                         const int off = row * 128 + ((((l16 >> 1) ^ (row & 7))) << 4) + (l16 & 1) * 8;
                         *reinterpret_cast<uint2 *>(a_hi + off) = oh;
@@ -437,7 +438,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 __syncwarp();
                 if (wl == 0) mbar_arrive(full_bar(s));
             }
-            if (rmax > 65504.f && P.a.flag) *P.a.flag = 1u;
+            if (!(rmax <= 65504.f) && P.a.flag) *P.a.flag = 1u;
         }
     } else if (warp >= 4) {
         // ===================== wgmma consumers (warpgroups 1, 2) =====================
@@ -747,6 +748,8 @@ static int g_force_block_n = 0;
 static int g_seg_chunks = 4;  // 64-channel slices per accumulation segment (4 -> 48 chained wgmma)
 static int g_pf = 4;          // L2 prefetch distance (K-slices) for flat operands; 0 = off
 static int g_xf_trunc = 1;
+static int g_last_dispatch = 0;
+int tc_last_dispatch() { return g_last_dispatch; }
 void tc_set_prefetch(int n) { g_pf = n < 0 ? 0 : n; }
 void tc_set_xf_trunc(int on) { g_xf_trunc = on; }
 void tc_set_block_n(int n) { g_force_block_n = n; }
@@ -888,6 +891,7 @@ static void launch_tm(const ConvParams &P, const TcPlan &plan, const TcGeom &G, 
     memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
     memcpy(&a2_hi, plan.tmap_a2_hi, 128); memcpy(&a2_lo, plan.tmap_a2_lo, 128);
     k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
+    g_last_dispatch = BLOCK_N | MODE << 8 | (XF ? 1 : 0) << 12 | (ONE ? 1 : 0) << 13;
 }
 
 template <int BLOCK_N, bool ONE>
