@@ -77,6 +77,132 @@ def _as_ids(a):
     return b
 
 
+def pack_images(imgs):
+    """RGB images [H_i,W_i,3] -> (uint8 [sum H_i*W_i*3] back to back in input order, shapes int32 [n,2] = (H_i, W_i)):
+    the input of hvn_infer_tiles."""
+    arrs = [np.ascontiguousarray(a, dtype=np.uint8) for a in imgs]
+    for a in arrs:
+        if a.ndim != 3 or a.shape[2] != 3:
+            raise ValueError("tile images must be RGB [H,W,3], got %s" % (a.shape,))
+    shapes = np.array([a.shape[:2] for a in arrs], dtype=np.int32).reshape(-1, 2)
+    packed = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else np.zeros((0,), np.uint8)
+    return packed, shapes
+
+
+def tiles_sizes(shapes):
+    """Default (rows_cap, pts_cap) of a tile group: hvn_infer_tile's per-image defaults, summed."""
+    px = [int(h) * int(w) for h, w in np.asarray(shapes).reshape(-1, 2)]
+    return sum(max(16, p // 64) for p in px), sum(max(4096, p // 16) for p in px)
+
+
+def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None):
+    """Packed outputs of hvn_infer_tiles -> one (pred [H,W,C] or None, inst [H,W], table [k,10], offs [k+1], pts [m,2]
+    or None) per image, the tuple Context.infer_tile returns: offs index the image's own points."""
+    out = []
+    p0 = 0
+    C = None if pred is None else pred.size // max(1, int(sum(int(h) * int(w) for h, w in shapes)))
+    for i, (h, w) in enumerate(np.asarray(shapes).reshape(-1, 2)):
+        h, w = int(h), int(w)
+        r0, r1 = int(row_offs[i]), int(row_offs[i + 1])
+        pm = None if pred is None else pred[p0 * C:(p0 + h * w) * C].reshape(h, w, C)
+        im = inst[p0:p0 + h * w].reshape(h, w)
+        offs = pt = None
+        if pt_offs is not None:
+            offs = np.asarray(pt_offs[r0:r1 + 1], dtype=np.int64) - int(pt_offs[r0])
+            pt = pts[int(pt_offs[r0]):int(pt_offs[r1])]
+        out.append((pm, im, table[r0:r1], offs, pt))
+        p0 += h * w
+    return out
+
+
+_TILES_ARGS = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+               ctypes.c_void_p]
+
+
+class TilesJob:
+    """A tile group enqueued with hvn_infer_tiles_dev (Context.infer_tiles_begin).  result() synchronises and returns
+    what Context.infer_tiles returns.  A capacity failure reruns the group through Context.infer_tiles with the sizes the
+    offsets report; a range failure reruns it there too, which raises act_shift."""
+
+    def __init__(self, ctx, imgs, patch_in, batch, want_pred, contours):
+        self.ctx, self.imgs, self.patch_in, self.batch = ctx, imgs, patch_in, batch
+        self.want_pred, self.contours = want_pred, contours
+        self.packed, self.shapes = pack_images(imgs)
+        n = self.shapes.shape[0]
+        px = int(self.packed.size // 3)
+        self.oc = ctx.out_shape(patch_in, patch_in)[2]
+        self.rows_cap, self.pts_cap = tiles_sizes(self.shapes)
+        sizes = {"img": px * 3, "pred": px * self.oc * 4 if want_pred else 0, "inst": px * 4,
+                 "table": self.rows_cap * ROW_LEN * 8, "ro": (n + 1) * 4,
+                 "po": (self.rows_cap + 1) * 4 if contours else 0, "pts": self.pts_cap * 8 if contours else 0}
+        self.d = {k: (ctx.malloc(b) if b else None) for k, b in sizes.items()}
+        try:
+            ctx.h2d(self.d["img"], self.packed, self.packed.nbytes)
+            L = lib()
+            L.hvn_infer_tiles_dev.argtypes = _TILES_ARGS
+            check(L.hvn_infer_tiles_dev(ctx._h, n, _ptr(self.d["img"]), _ptr(self.shapes), int(patch_in), int(batch),
+                                        _ptr(self.d["pred"]), _ptr(self.d["inst"]), _ptr(self.d["table"]),
+                                        int(self.rows_cap), _ptr(self.d["ro"]), _ptr(self.d["pts"]),
+                                        int(self.pts_cap if contours else 0), _ptr(self.d["po"])))
+        except Exception:
+            self._free()
+            raise
+
+    def _free(self):
+        for k, p in self.d.items():
+            if p:
+                self.ctx.free(p)
+        self.d = {}
+
+    def result(self):
+        ctx, n = self.ctx, self.shapes.shape[0]
+        try:
+            try:
+                ctx.sync()
+            except HvnError as e:
+                if e.code != -6:
+                    raise
+                return self._rerun()
+            ro = np.zeros((n + 1,), dtype=np.int32)
+            ctx.d2h(ro, self.d["ro"], ro.nbytes)
+            rows = int(ro[-1])
+            po = None
+            if self.contours:
+                po = np.zeros((self.rows_cap + 1,), dtype=np.int32)
+                if rows <= self.rows_cap:
+                    ctx.d2h(po, self.d["po"], po.nbytes)
+            if rows > self.rows_cap:
+                return self._rerun(rows_cap=rows)  # the points are sized on the rerun's own retry if need be
+            if po is not None and int(po[rows]) > self.pts_cap:
+                return self._rerun(rows_cap=self.rows_cap, pts_cap=int(po[rows]))
+            px = int(self.packed.size // 3)
+            inst = np.empty((px,), dtype=np.int32)
+            ctx.d2h(inst, self.d["inst"], inst.nbytes)
+            table = np.empty((rows, ROW_LEN), dtype=np.int64)
+            if rows:
+                ctx.d2h(table, self.d["table"], table.nbytes)
+            pred = pts = None
+            if self.want_pred:
+                pred = np.empty((px * self.oc,), dtype=np.float32)
+                ctx.d2h(pred, self.d["pred"], pred.nbytes)
+            if self.contours:
+                pts = np.empty((int(po[rows]), 2), dtype=np.int32)
+                if pts.size:
+                    ctx.d2h(pts, self.d["pts"], pts.nbytes)
+                po = po[: rows + 1]
+            ctx.sync()
+            return split_tiles(self.shapes, inst, table, ro, pred, pts, po)
+        finally:
+            self._free()
+
+    def _rerun(self, rows_cap=None, pts_cap=None):
+        """The group again through the synchronising host variant, with the exact sizes when a capacity check failed."""
+        self._free()
+        return self.ctx.infer_tiles(self.imgs, self.patch_in, self.batch, want_pred=self.want_pred, contours=self.contours,
+                                    rows_cap=rows_cap, pts_cap=pts_cap)
+
+
 class Context:
     """One libhvn context (one device, one stream).  precision: "highest" (default; fp16 hi + lo operands, three
     products per MAC) or "high" (hi only, one fp16 product per MAC -- TF32-class operand precision); model contexts
@@ -323,6 +449,14 @@ class Context:
         check(L.hvn_valid_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
                               _ptr(d_counts), _ptr(d_sse), _ptr(d_flags)))
 
+    def mem_get_info(self):
+        """(free, total) device bytes of this context's device (hvn_mem_info)."""
+        free, total = ctypes.c_size_t(), ctypes.c_size_t()
+        L = lib()
+        L.hvn_mem_info.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)]
+        check(L.hvn_mem_info(self._h, ctypes.byref(free), ctypes.byref(total)))
+        return int(free.value), int(total.value)
+
     def tile_grid(self, H, W, patch_in):
         r, c = ctypes.c_int(), ctypes.c_int()
         check(lib().hvn_tile_grid(self._h, int(H), int(W), int(patch_in), ctypes.byref(r), ctypes.byref(c)))
@@ -363,6 +497,59 @@ class Context:
             n = int(nrows[0])
             return pred, inst, table[:n], offs, (pts[: int(offs[-1])] if contours else None)
         raise HvnError(-4, "infer_tile: capacity retries exhausted")
+
+    def infer_tiles(self, imgs, patch_in, batch=0, want_pred=True, contours=True, rows_cap=None, pts_cap=None):
+        """A group of RGB images [H_i,W_i,3] of any sizes through the device tile path in one stream of batches
+        (hvn_infer_tiles).  Returns one (pred or None, inst, table [k,10], offs or None, pts or None) per image, each
+        equal to infer_tile on that image alone."""
+        packed, shapes = pack_images(imgs)
+        n = shapes.shape[0]
+        if n < 1:
+            raise ValueError("infer_tiles needs at least one image")
+        px = int(packed.size // 3)
+        _, _, oc = self.out_shape(patch_in, patch_in)
+        r0, p0 = tiles_sizes(shapes)
+        rows_cap = r0 if rows_cap is None else int(rows_cap)
+        pts_cap = p0 if pts_cap is None else int(pts_cap)
+        L = lib()
+        L.hvn_infer_tiles.argtypes = _TILES_ARGS
+        for _attempt in range(4):  # at most: grow the table once, then the point buffer once
+            pred = np.empty((px * oc,), dtype=np.float32) if want_pred else None
+            inst = np.empty((px,), dtype=np.int32)
+            table = np.empty((rows_cap, ROW_LEN), dtype=np.int64)
+            ro = np.zeros((n + 1,), dtype=np.int32)
+            po = np.zeros((rows_cap + 1,), dtype=np.int32) if contours else None
+            pts = np.empty((pts_cap, 2), dtype=np.int32) if contours else None
+            rc = self._retry_range(lambda: L.hvn_infer_tiles(
+                self._h, n, _ptr(packed), _ptr(shapes), int(patch_in), int(batch), _ptr(pred), _ptr(inst), _ptr(table),
+                int(rows_cap), _ptr(ro), _ptr(pts), int(pts_cap if contours else 0), _ptr(po)))
+            if rc == -4:  # HVN_ERR_CAPACITY: retry with the exact size the offsets report
+                if int(ro[-1]) > rows_cap:
+                    rows_cap = int(ro[-1])
+                else:
+                    pts_cap = int(po[int(ro[-1])])
+                continue
+            check(rc)
+            rows = int(ro[-1])
+            if contours:
+                po = po[: rows + 1]
+                pts = pts[: int(po[-1])]
+            return split_tiles(shapes, inst, table[:rows], ro, pred, pts, po)
+        raise HvnError(-4, "infer_tiles: capacity retries exhausted")
+
+    def infer_tiles_begin(self, imgs, patch_in, batch=0, want_pred=True, contours=True):
+        """Enqueues a tile group with hvn_infer_tiles_dev and returns at once; TilesJob.result() waits for it."""
+        return TilesJob(self, list(imgs), patch_in, batch, want_pred, contours)
+
+    def infer_tiles_dev(self, n, d_imgs, shapes, patch_in, batch, d_pred, d_inst, d_table, rows_cap, d_row_offs, d_pts,
+                        pts_cap, d_pt_offs):
+        """hvn_infer_tiles_dev on device pointers (shapes: host int32 [n,2]); stream-ordered, no synchronisation."""
+        L = lib()
+        L.hvn_infer_tiles_dev.argtypes = _TILES_ARGS
+        sh = np.ascontiguousarray(shapes, dtype=np.int32)
+        check(L.hvn_infer_tiles_dev(self._h, int(n), _ptr(d_imgs), _ptr(sh), int(patch_in), int(batch), _ptr(d_pred),
+                                    _ptr(d_inst), _ptr(d_table), int(rows_cap), _ptr(d_row_offs), _ptr(d_pts),
+                                    int(pts_cap), _ptr(d_pt_offs)))
 
     def tile_predict_dev(self, d_img, H, W, patch_in, cell_lo, cell_hi, batch, d_pred):
         L = lib()

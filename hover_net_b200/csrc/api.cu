@@ -1,4 +1,5 @@
 // C ABI of libhvn (include/hvn.h).  Thin: argument checks, host<->device staging, error mapping.
+#include <algorithm>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -25,6 +26,11 @@ struct hvn_ctx {
     Arena stats_arena;             // pair-table workspace of hvn_inst_pairs*
     Arena targets_arena;           // workspace of hvn_targets* and hvn_valid*
     Arena valid_arena;             // maps and counts of hvn_valid*
+    Arena group_arena;             // slot table, padded instance tables and slot-order maps of the tile-group path
+    void *pin = nullptr;           // pinned staging of the tile-group slot table (uploaded stream-ordered)
+    size_t pin_bytes = 0;
+    cudaEvent_t pin_ev = nullptr;  // recorded after the last upload from `pin`
+    long long group_table_rows = 0;  // padded instance-table rows the last tile group took from group_arena
     int chunk = 0;
     int profile = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -79,6 +85,7 @@ static int create_common(int device, hvn_ctx **out, const char *mode, int nr_typ
     HVN_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     for (auto &e : c->ev) HVN_CUDA(cudaEventCreate(&e));
     for (auto &e : c->tev) HVN_CUDA(cudaEventCreate(&e));
+    HVN_CUDA(cudaEventCreateWithFlags(&c->pin_ev, cudaEventDisableTiming));
     *out = c.release();
     API_END
 }
@@ -98,6 +105,9 @@ void hvn_destroy(hvn_ctx *c) {
     c->stats_arena.release();
     c->targets_arena.release();
     c->valid_arena.release();
+    c->group_arena.release();
+    if (c->pin) cudaFreeHost(c->pin);
+    if (c->pin_ev) cudaEventDestroy(c->pin_ev);
     for (auto &e : c->ev) cudaEventDestroy(e);
     for (auto &e : c->tev) cudaEventDestroy(e);
     cudaStreamDestroy(c->stream);
@@ -182,6 +192,7 @@ int64_t hvn_get_counter(const hvn_ctx *c, const char *key) {
     if (k == "kernel_launches") return (c->model ? c->model->kernel_launches : 0) + c->pp_launches;
     if (k == "tc_launches") return c->model ? c->model->tc_launches : 0;
     if (k == "pp_launches") return c->pp_launches;
+    if (k == "tile_table_rows") return c->group_table_rows;
     if (c->model) {
         if (k == "last_flops") return (int64_t)c->model->last_flops;
         if (k.rfind("launches:", 0) == 0) { auto it = c->model->class_launches.find(k.substr(9)); return it == c->model->class_launches.end() ? 0 : it->second; }
@@ -414,13 +425,155 @@ int hvn_tile_grid(const hvn_ctx *c, int H, int W, int patch_in, int *rows, int *
     API_END
 }
 
-static int run_tile_predict(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, int lo, int hi, int batch, float *pred) {
+// A group of images laid out for the tile path (tile_plan): slot order groups equal sizes, `identity` when that is the
+// input order already.
+struct TileGroup {
+    std::vector<TileImage> slots;
+    std::vector<int> slot_of;
+    int n = 0, oc = 0;
+    long long table_rows = 0;  // rows of the group's padded instance tables (sum of the slots' max_rows)
+    size_t px = 0;         // pixels of the whole group
+    long long cells = 0;   // patches of the whole group
+    bool identity = true;
+};
+
+static void plan_tiles(hvn_ctx *c, int n, const int32_t *shapes, int patch_in, long long rows_cap, TileGroup &g) {
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    HVN_CHECK(n >= 1 && shapes, HVN_ERR_INVALID, "a tile group needs n_images >= 1 and their shapes");
+    HVN_CHECK(rows_cap >= 1 && rows_cap < (1ll << 31) - 1, HVN_ERR_INVALID, "rows_cap must be in 1 .. 2^31 - 2");
+    int oh, ow;
+    c->model->out_shape(patch_in, patch_in, oh, ow, g.oc);
+    HVN_CHECK(oh == ow && oh >= 1, HVN_ERR_INVALID, "unsupported patch size for this model mode");
+    tile_plan(shapes, n, oh, g.oc, g.slots, g.slot_of);
+    g.n = n;
+    for (int i = 0; i < n; ++i) {
+        g.px += (size_t)g.slots[i].H * g.slots[i].W;
+        g.cells += (long long)g.slots[i].rows * g.slots[i].cols;
+        g.identity = g.identity && g.slot_of[i] == i;
+    }
+    // each slot's padded table holds min(rows_cap, its own id bound) rows -- no map has more rows than its id bound,
+    // and a map with more than rows_cap rows makes the packed table overflow anyway -- so the tables take about 14 B
+    // per pixel of the group whatever its mix of sizes; equal sizes share a stride, as one postproc_run needs
+    for (auto &t : g.slots) {
+        t.max_rows = (int)std::min<long long>(rows_cap, postproc_max_ids(t.H, t.W));
+        t.row0 = g.table_rows;
+        g.table_rows += t.max_rows;
+    }
+}
+
+// Uploads the slot table through the context's pinned buffer, stream-ordered: no host synchronisation beyond waiting
+// for the previous upload to have left the buffer.
+static void upload_slots(hvn_ctx *c, const TileGroup &g, TileImage *d_slots, int *d_slot_of) {
+    const size_t tb = g.slots.size() * sizeof(TileImage), bytes = tb + (size_t)g.n * sizeof(int);
+    HVN_CUDA(cudaEventSynchronize(c->pin_ev));
+    if (bytes > c->pin_bytes) {
+        if (c->pin) HVN_CUDA(cudaFreeHost(c->pin));
+        c->pin = nullptr;
+        c->pin_bytes = 0;
+        HVN_CUDA(cudaMallocHost(&c->pin, bytes));
+        c->pin_bytes = bytes;
+    }
+    std::memcpy(c->pin, g.slots.data(), tb);
+    HVN_CUDA(cudaMemcpyAsync(d_slots, c->pin, tb, cudaMemcpyHostToDevice, c->stream));
+    if (d_slot_of) {
+        std::memcpy((char *)c->pin + tb, g.slot_of.data(), (size_t)g.n * sizeof(int));
+        HVN_CUDA(cudaMemcpyAsync(d_slot_of, (char *)c->pin + tb, (size_t)g.n * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    }
+    HVN_CUDA(cudaEventRecord(c->pin_ev, c->stream));
+}
+
+static int run_tile_predict(hvn_ctx *c, const uint8_t *imgs, const TileImage *d_slots, int n, long long lo, long long hi,
+                            int patch_in, int batch, float *pred) {
     int oh, ow, oc;
     c->model->out_shape(patch_in, patch_in, oh, ow, oc);
     if (batch < 1) batch = 64;
+    batch = std::min(batch, 65535);
     c->tile_arena.reset();
     c->tile_arena.reserve(tile_workspace_bytes(patch_in, oh, oc, batch) + 1024);
-    return tile_predict(*c->model, c->tile_arena, c->stream, img, H, W, patch_in, lo, hi, batch, c->chunk, pred);
+    return tile_predict(*c->model, c->tile_arena, c->stream, imgs, d_slots, n, lo, hi, patch_in, batch, c->chunk, pred);
+}
+
+// The device work of a tile group, enqueued on the context stream: patches of every image in one stream of batches,
+// then per size class one post-processing call over its maps and one contour count, then the packed tables
+// (input order) and -- when pt_offs is not null -- the packed contour points.  pred / inst are slot-ordered maps; null
+// takes them from the context's workspace.  *pred_out / *inst_out receive the maps that were written.
+static void run_tiles(hvn_ctx *c, const TileGroup &g, const uint8_t *imgs, int patch_in, int batch, float *pred,
+                      int32_t *inst, int64_t *table, long long rows_cap, int32_t *row_offs, int32_t *pts, long long pts_cap,
+                      int32_t *pt_offs, float **pred_out, int32_t **inst_out) {
+    const int n = g.n, nt = c->model->nr_types;
+    const size_t R = (size_t)g.table_rows;
+    const bool contours = pt_offs != nullptr, one = n == 1;
+    // a group of one writes its table and its point counts in place (the packing is the identity)
+    const size_t ws = (size_t)n * sizeof(TileImage) + (size_t)n * 8 + (one ? 0 : R * 80) + (contours && !one ? R * 4 : 0) +
+                      (pred ? 0 : g.px * g.oc * 4) + (inst ? 0 : g.px * 4) + 8 * 256;
+    c->group_table_rows = one ? 0 : (long long)R;
+    c->group_arena.reset();
+    c->group_arena.reserve(ws);
+    TileImage *d_slots = c->group_arena.take<TileImage>(n);
+    int *d_slot_of = c->group_arena.take<int>(n);
+    int *d_nrows = c->group_arena.take<int>(n);
+    long long *pad = one ? (long long *)table : c->group_arena.take<long long>(R * 10);
+    int *cnt = !contours ? nullptr : (one ? pt_offs : c->group_arena.take<int>(R));
+    if (!pred) pred = c->group_arena.take<float>(g.px * g.oc);
+    if (!inst) inst = c->group_arena.take<int32_t>(g.px);
+    *pred_out = pred;
+    *inst_out = inst;
+    upload_slots(c, g, d_slots, d_slot_of);
+
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
+    c->model->kernel_launches += run_tile_predict(c, imgs, d_slots, n, 0, g.cells, patch_in, batch, pred);
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[1], c->stream));
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[2], c->stream));
+    if (contours) HVN_CUDA(cudaMemsetAsync(pt_offs, 0, (size_t)(rows_cap + 1) * 4, c->stream));
+    std::vector<std::pair<int, int>> classes;  // (first slot, maps) of each size class
+    for (int s = 0; s < n; ++s) {
+        if (s && g.slots[s].H == g.slots[s - 1].H && g.slots[s].W == g.slots[s - 1].W) ++classes.back().second;
+        else classes.push_back({s, 1});
+    }
+    for (auto &k : classes) {
+        const TileImage &t = g.slots[k.first];
+        const size_t p0 = (size_t)(t.pred_off / g.oc);
+        c->pp_launches += postproc_run(c->pp_arena, c->stream, pred + t.pred_off, k.second, t.H, t.W, g.oc, nt, inst + p0,
+                                       pad + (size_t)t.row0 * 10, t.max_rows, d_nrows + k.first,
+                                       c->profile >= 3 ? &c->pp_log : nullptr);
+        if (contours)
+            c->pp_launches += contours_count(c->stream, inst + p0, pad + (size_t)t.row0 * 10, d_nrows + k.first, k.second,
+                                             t.H, t.W, t.max_rows, cnt + t.row0);
+    }
+    c->pp_launches += pack_tables(c->stream, pad, d_nrows, n, 0, (long long *)table, rows_cap, row_offs, d_slot_of,
+                                  d_slots, cnt, pt_offs);
+    if (contours) {
+        c->pp_launches += contours_scan(c->stream, pt_offs, (int)rows_cap);
+        for (auto &k : classes) {
+            const TileImage &t = g.slots[k.first];
+            c->pp_launches += contours_write_packed(c->stream, inst + t.pred_off / g.oc, pad + (size_t)t.row0 * 10,
+                                                    d_nrows + k.first, k.second, t.H, t.W, t.max_rows, d_slots + k.first, row_offs,
+                                                    n, rows_cap, pt_offs, pts, pts_cap);
+        }
+    }
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[3], c->stream));
+}
+
+// Copies slot-ordered maps (elem_px bytes per pixel) to dst in input order.
+static void copy_maps(hvn_ctx *c, const TileGroup &g, void *dst, const void *src, size_t elem_px, cudaMemcpyKind kind) {
+    if (g.identity) {
+        HVN_CUDA(cudaMemcpyAsync(dst, src, g.px * elem_px, kind, c->stream));
+        return;
+    }
+    size_t o = 0;
+    for (int i = 0; i < g.n; ++i) {
+        const TileImage &t = g.slots[g.slot_of[i]];
+        const size_t b = (size_t)t.H * t.W * elem_px;
+        HVN_CUDA(cudaMemcpyAsync((char *)dst + o, (const char *)src + (size_t)(t.pred_off / g.oc) * elem_px, b, kind, c->stream));
+        o += b;
+    }
+}
+
+static void check_tiles_args(hvn_ctx *c, const void *imgs, const void *inst, const void *table, const void *row_offs,
+                             const void *pts, long long pts_cap, const void *pt_offs) {
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    HVN_CHECK(imgs && inst && table && row_offs, HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(pts_cap >= 0 && (!pt_offs || pts || pts_cap == 0), HVN_ERR_INVALID, "contours requested without a point buffer");
 }
 
 int hvn_tile_predict_dev(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, int cell_lo, int cell_hi, int batch,
@@ -429,8 +582,16 @@ int hvn_tile_predict_dev(hvn_ctx *c, const uint8_t *img, int H, int W, int patch
     use(c);
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     HVN_CHECK(img && pred && H >= 1 && W >= 1, HVN_ERR_INVALID, "bad argument");
+    const int32_t shape[2] = {H, W};
+    TileGroup g;
+    plan_tiles(c, 1, shape, patch_in, 1, g);
+    HVN_CHECK(cell_lo >= 0 && cell_hi <= g.cells && cell_lo <= cell_hi, -1, "patch range outside the grid");
+    c->group_arena.reset();
+    c->group_arena.reserve(1024);
+    TileImage *d_slots = c->group_arena.take<TileImage>(1);
+    upload_slots(c, g, d_slots, nullptr);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
-    c->model->kernel_launches += run_tile_predict(c, img, H, W, patch_in, cell_lo, cell_hi, batch, pred);
+    c->model->kernel_launches += run_tile_predict(c, img, d_slots, 1, cell_lo, cell_hi, patch_in, batch, pred);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[1], c->stream));
     finish_profile(c, true, false);
     API_END
@@ -443,9 +604,10 @@ int hvn_infer_tile(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, i
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     HVN_CHECK(img && inst && table && n_rows && H >= 1 && W >= 1 && max_rows >= 1, HVN_ERR_INVALID, "bad argument");
     HVN_CHECK(!offs || pts || cap == 0, HVN_ERR_INVALID, "contours requested without a point buffer");
-    int oh, ow, oc, rows, cols;
-    c->model->out_shape(patch_in, patch_in, oh, ow, oc);
-    tile_grid(H, W, oh, &rows, &cols);
+    const int32_t shape[2] = {H, W};
+    TileGroup g;
+    plan_tiles(c, 1, shape, patch_in, max_rows, g);
+    const int oc = g.oc;
     const size_t px = (size_t)H * W, tb = (size_t)max_rows * HVN_ROW_LEN, no = (size_t)max_rows + 1;
     if (!offs) cap = 0;
     c->io_arena.reset();
@@ -455,23 +617,23 @@ int hvn_infer_tile(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, i
     int32_t *d_inst = c->io_arena.take<int32_t>(px);
     int64_t *d_tab = c->io_arena.take<int64_t>(tb);
     HVN_CUDA(cudaMemsetAsync(d_tab, 0, tb * 8, c->stream));  // rows past n_rows go back to the caller as zeros
-    int32_t *d_nr = c->io_arena.take<int32_t>(1);
-    int32_t *d_offs = c->io_arena.take<int32_t>(no);
+    int32_t *d_ro = c->io_arena.take<int32_t>(2);
+    int32_t *d_offs = offs ? c->io_arena.take<int32_t>(no) : nullptr;
     int32_t *d_pts = c->io_arena.take<int32_t>((size_t)cap * 2 + 2);
     HVN_CUDA(cudaMemcpyAsync(d_img, img, px * 3, cudaMemcpyHostToDevice, c->stream));
-    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
-    c->model->kernel_launches += run_tile_predict(c, d_img, H, W, patch_in, 0, rows * cols, batch, d_pred);
-    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[1], c->stream));
-    run_postproc(c, d_pred, 1, H, W, oc, c->model->nr_types, d_inst, d_tab, max_rows, d_nr);
-    if (offs) c->pp_launches += contours_run(c->stream, d_inst, (const long long *)d_tab, d_nr, 1, H, W, max_rows, d_pts, cap, d_offs);
+    float *wp;
+    int32_t *wi;
+    run_tiles(c, g, d_img, patch_in, batch, d_pred, d_inst, d_tab, max_rows, d_ro, d_pts, cap, d_offs, &wp, &wi);
+    int32_t ro[2] = {0, 0};
     if (pred) HVN_CUDA(cudaMemcpyAsync(pred, d_pred, px * oc * 4, cudaMemcpyDeviceToHost, c->stream));
     HVN_CUDA(cudaMemcpyAsync(inst, d_inst, px * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(n_rows, d_nr, 4, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(ro, d_ro, 8, cudaMemcpyDeviceToHost, c->stream));
     HVN_CUDA(cudaMemcpyAsync(table, d_tab, tb * 8, cudaMemcpyDeviceToHost, c->stream));
     if (offs) HVN_CUDA(cudaMemcpyAsync(offs, d_offs, no * 4, cudaMemcpyDeviceToHost, c->stream));
     HVN_CUDA(cudaStreamSynchronize(c->stream));
     finish_profile(c, true, true);
     check_range(c);
+    n_rows[0] = ro[1];
     check_rows(n_rows, 1, max_rows);
     if (offs) {
         const long long total = offs[no - 1];
@@ -481,6 +643,71 @@ int hvn_infer_tile(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, i
             HVN_CUDA(cudaStreamSynchronize(c->stream));
         }
     }
+    API_END
+}
+
+int hvn_infer_tiles(hvn_ctx *c, int n, const uint8_t *imgs, const int32_t *shapes, int patch_in, int batch, float *pred,
+                    int32_t *inst, int64_t *table, int64_t rows_cap, int32_t *row_offs, int32_t *pts, int64_t pts_cap,
+                    int32_t *pt_offs) {
+    API_BEGIN
+    use(c);
+    check_tiles_args(c, imgs, inst, table, row_offs, pts, pts_cap, pt_offs);
+    TileGroup g;
+    plan_tiles(c, n, shapes, patch_in, rows_cap, g);
+    if (!pt_offs) pts_cap = 0;
+    const size_t px = g.px, no = pt_offs ? (size_t)rows_cap + 1 : 0;
+    c->io_arena.reset();
+    c->io_arena.reserve(px * 3 + px * g.oc * 4 + px * 4 + (size_t)rows_cap * 80 + (size_t)(n + 1) * 4 + no * 4 +
+                        (size_t)pts_cap * 8 + 16384);
+    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
+    float *d_pred = c->io_arena.take<float>(px * g.oc);
+    int32_t *d_inst = c->io_arena.take<int32_t>(px);
+    int64_t *d_tab = c->io_arena.take<int64_t>((size_t)rows_cap * HVN_ROW_LEN);
+    int32_t *d_ro = c->io_arena.take<int32_t>((size_t)n + 1);
+    int32_t *d_po = pt_offs ? c->io_arena.take<int32_t>(no) : nullptr;
+    int32_t *d_pts = c->io_arena.take<int32_t>((size_t)pts_cap * 2 + 2);
+    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
+    float *wp;
+    int32_t *wi;
+    run_tiles(c, g, d_imgs, patch_in, batch, d_pred, d_inst, d_tab, rows_cap, d_ro, d_pts, pts_cap, d_po, &wp, &wi);
+    if (pred) copy_maps(c, g, pred, d_pred, (size_t)g.oc * 4, cudaMemcpyDeviceToHost);
+    copy_maps(c, g, inst, d_inst, 4, cudaMemcpyDeviceToHost);
+    HVN_CUDA(cudaMemcpyAsync(row_offs, d_ro, (size_t)(n + 1) * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (pt_offs) HVN_CUDA(cudaMemcpyAsync(pt_offs, d_po, no * 4, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    finish_profile(c, true, true);
+    check_range(c);
+    const long long rows = row_offs[n];
+    HVN_CHECK(rows <= rows_cap, HVN_ERR_CAPACITY,
+              "instance table too small: " + std::to_string(rows) + " rows, rows_cap=" + std::to_string(rows_cap));
+    if (rows > 0) HVN_CUDA(cudaMemcpyAsync(table, d_tab, (size_t)rows * 80, cudaMemcpyDeviceToHost, c->stream));
+    if (pt_offs) {
+        const long long total = pt_offs[rows];
+        HVN_CHECK(total <= pts_cap, HVN_ERR_CAPACITY,
+                  "contour buffer too small: " + std::to_string(total) + " points, pts_cap=" + std::to_string(pts_cap));
+        if (total > 0) HVN_CUDA(cudaMemcpyAsync(pts, d_pts, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
+    }
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    API_END
+}
+
+int hvn_infer_tiles_dev(hvn_ctx *c, int n, const uint8_t *imgs, const int32_t *shapes, int patch_in, int batch,
+                        float *pred, int32_t *inst, int64_t *table, int64_t rows_cap, int32_t *row_offs, int32_t *pts,
+                        int64_t pts_cap, int32_t *pt_offs) {
+    API_BEGIN
+    use(c);
+    check_tiles_args(c, imgs, inst, table, row_offs, pts, pts_cap, pt_offs);
+    TileGroup g;
+    plan_tiles(c, n, shapes, patch_in, rows_cap, g);
+    if (!pt_offs) pts_cap = 0;
+    // the caller's maps are in input order: written in place when that is the slot order, else copied from the
+    // context's slot-order maps afterwards
+    float *wp;
+    int32_t *wi;
+    run_tiles(c, g, imgs, patch_in, batch, g.identity ? pred : nullptr, g.identity ? inst : nullptr, table, rows_cap,
+              row_offs, pts, pts_cap, pt_offs, &wp, &wi);
+    if (pred && wp != pred) copy_maps(c, g, pred, wp, (size_t)g.oc * 4, cudaMemcpyDeviceToDevice);
+    if (wi != inst) copy_maps(c, g, inst, wi, 4, cudaMemcpyDeviceToDevice);
     API_END
 }
 
@@ -714,6 +941,13 @@ int hvn_pack_tables_dev(hvn_ctx *c, const int64_t *table, const int32_t *n_rows,
     use(c);
     HVN_CHECK(table && n_rows && packed && offs && n >= 1 && max_rows >= 1 && cap >= 0, HVN_ERR_INVALID, "bad argument");
     c->pp_launches += pack_tables(c->stream, (const long long *)table, n_rows, n, max_rows, (long long *)packed, cap, offs);
+    API_END
+}
+int hvn_mem_info(hvn_ctx *c, size_t *free_bytes, size_t *total_bytes) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(free_bytes && total_bytes, HVN_ERR_INVALID, "null out pointer");
+    HVN_CUDA(cudaMemGetInfo(free_bytes, total_bytes));
     API_END
 }
 int hvn_get_stream(hvn_ctx *c, void **stream) {

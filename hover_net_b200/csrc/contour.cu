@@ -11,6 +11,7 @@
 // changes.  A flood region is 4-connected, hence a single 8-connected component whose outer border is the
 // first contour cv2 returns.
 #include "postproc.h"
+#include "tile.h"
 
 namespace hvn {
 namespace {
@@ -87,6 +88,27 @@ __global__ void k_contour_trace(const int *__restrict__ inst_all, const long lon
     }
 }
 
+// Write pass of a size class of a tile group into the packed layout: padded map m of the class is output image
+// img_of[m] (a TileImage slot table, read at .img); its row r is packed row row_offs[img] + r, whose points are
+// pts[pt_offs[row] : pt_offs[row + 1]].  Nothing is written when the packed table did not fit (row_offs[n_out] >
+// rows_cap) or a row's points do not fit in cap.
+__global__ void k_contour_write_packed(const int *__restrict__ inst_all, const long long *__restrict__ table,
+                                       const int *__restrict__ n_rows, int n_maps, int H, int W, int max_rows,
+                                       const TileImage *__restrict__ img_of, const int *__restrict__ row_offs, int n_out,
+                                       long long rows_cap, const int *__restrict__ pt_offs, int *__restrict__ pts,
+                                       long long cap) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n_maps * max_rows || row_offs[n_out] > rows_cap) return;
+    const int m = idx / max_rows, r = idx - m * max_rows;
+    if (r >= min(n_rows[m], max_rows)) return;
+    const long long row = (long long)row_offs[img_of[m].img] + r;
+    const long long o = pt_offs[row], n = pt_offs[row + 1] - o;
+    if (n <= 0 || o + n > cap) return;
+    const long long *t = table + (size_t)idx * 10;
+    Box b = {(int)t[1], (int)t[2], (int)t[3], (int)t[4]};
+    trace<true>(inst_all + (size_t)m * H * W, W, (int)t[0], b, pts + 2 * o);
+}
+
 // counts[0..total) -> exclusive prefix in place, offs[total] = sum.  One block.
 __global__ void __launch_bounds__(1024) k_contour_scan(int *__restrict__ offs, int total) {
     __shared__ int part[1024];
@@ -114,12 +136,35 @@ __global__ void __launch_bounds__(1024) k_contour_scan(int *__restrict__ offs, i
 
 }  // namespace
 
+int contours_count(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps, int H,
+                   int W, int max_rows, int *cnt) {
+    k_contour_trace<false><<<cdiv((long long)n_maps * max_rows, 128), 128, 0, stream>>>(inst, table, n_rows, n_maps, H, W,
+                                                                                      max_rows, cnt, nullptr, 0);
+    HVN_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int contours_scan(cudaStream_t stream, int *offs, int total) {
+    k_contour_scan<<<1, 1024, 0, stream>>>(offs, total);
+    HVN_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int contours_write_packed(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps,
+                          int H, int W, int max_rows, const TileImage *img_of, const int *row_offs, int n_out,
+                          long long rows_cap, const int *pt_offs, int *pts, long long cap) {
+    k_contour_write_packed<<<cdiv((long long)n_maps * max_rows, 128), 128, 0, stream>>>(
+        inst, table, n_rows, n_maps, H, W, max_rows, img_of, row_offs, n_out, rows_cap, pt_offs, pts, cap);
+    HVN_CUDA(cudaGetLastError());
+    return 1;
+}
+
 int contours_run(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps, int H,
                  int W, int max_rows, int *pts, long long cap, int *offs) {
     const int total = n_maps * max_rows;
     const int threads = 128, blocks = cdiv(total, threads);
-    k_contour_trace<false><<<blocks, threads, 0, stream>>>(inst, table, n_rows, n_maps, H, W, max_rows, offs, nullptr, 0);
-    k_contour_scan<<<1, 1024, 0, stream>>>(offs, total);
+    contours_count(stream, inst, table, n_rows, n_maps, H, W, max_rows, offs);
+    contours_scan(stream, offs, total);
     k_contour_trace<true><<<blocks, threads, 0, stream>>>(inst, table, n_rows, n_maps, H, W, max_rows, offs, pts, cap);
     HVN_CUDA(cudaGetLastError());
     return 3;

@@ -1057,7 +1057,7 @@ template <typename A>
 static void pp_layout(A &ar, PostprocBuffers &b, int n, int H, int W, int nr_types) {
     size_t N = (size_t)H * W, T = (size_t)n * N;
     b.max_blobs = (int)(N / 10 + 1);
-    b.max_ids = (int)(N / 6 + 8);
+    b.max_ids = postproc_max_ids(H, W);
     b.stats = ar.template take<PPStats>(n);
     b.fg = ar.template take<unsigned char>(T);
     b.L1 = ar.template take<int>(T);
@@ -1083,6 +1083,8 @@ static void pp_layout(A &ar, PostprocBuffers &b, int n, int H, int W, int nr_typ
     b.acc = ar.template take<InstAcc>((size_t)n * b.max_ids);
     b.tcnt = ar.template take<int>((size_t)n * b.max_ids * (nr_types > 0 ? nr_types : 1));
 }
+
+int postproc_max_ids(int H, int W) { return (int)((size_t)H * W / 6 + 8); }
 
 size_t postproc_workspace_bytes(int n, int H, int W, int nr_types) {
     ArenaSizer s;

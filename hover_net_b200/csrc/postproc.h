@@ -20,6 +20,8 @@ struct PostprocBuffers {
 
 void postproc_set_flood_impl(int v);  // test hook: 0 auto, 1 shared-memory heap, 2 global-memory heap
 size_t postproc_workspace_bytes(int n, int H, int W, int nr_types);
+// Instance ids a map can hold (ids 1 .. postproc_max_ids - 1): an upper bound on the table rows of one H x W map.
+int postproc_max_ids(int H, int W);
 
 // pred [n,H,W,C] f32 (device) -> inst [n,H,W] i32, table [n,max_rows,10] i64, n_rows [n] i32 (device).
 // Returns the number of kernels launched on `stream`.
@@ -31,5 +33,16 @@ int postproc_run(Arena &arena, cudaStream_t stream, const float *pred, int n, in
 // of kernels launched.
 int contours_run(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps, int H,
                  int W, int max_rows, int *pts, long long cap, int *offs);
+// The three phases of contours_run, for the packed layout of a tile group: per-row point counts cnt [n*max_rows]
+// (0 past n_rows); exclusive scan of offs [0, total) in place, offs[total] = sum; and the write pass of one size class
+// at its packed positions (row r of class map m is packed row row_offs[img_of[m].img] + r, its points
+// pts[pt_offs[row] : pt_offs[row+1]]; nothing is written when row_offs[n_out] > rows_cap or past cap).
+struct TileImage;
+int contours_count(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps, int H,
+                   int W, int max_rows, int *cnt);
+int contours_scan(cudaStream_t stream, int *offs, int total);
+int contours_write_packed(cudaStream_t stream, const int *inst, const long long *table, const int *n_rows, int n_maps,
+                          int H, int W, int max_rows, const TileImage *img_of, const int *row_offs, int n_out,
+                          long long rows_cap, const int *pt_offs, int *pts, long long cap);
 
 }  // namespace hvn

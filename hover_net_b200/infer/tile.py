@@ -1,17 +1,21 @@
 """Drop-in for reference `infer/tile.py` (SURVEY.md row f1): `InferManager.process_file_list(run_args)`
 with the reference's run_args, patch geometry, stitching, and `.mat` / `.json` / overlay / QuPath outputs.
 
-What changes underneath: patches go to the device in batches through `infer_step` (libhvn), the
-stitched map is post-processed by the device `process` in this process (the reference's
-`nr_post_proc_workers` pool and `nr_inference_workers` loader processes are accepted and ignored --
-there is no CPU stage left to parallelise), and files are handled one at a time instead of being
-cached by a RAM budget (`mem_usage` is accepted for compatibility)."""
+What changes underneath: patches go to the device in batches through libhvn, the stitched maps are post-processed by
+the device `process` in this process (the reference's `nr_post_proc_workers` pool and `nr_inference_workers` loader
+processes are accepted and ignored -- there is no CPU stage left to parallelise).  Files are cached in groups by the
+reference's RAM budget (`mem_usage` of the available RAM, `sys.getsizeof(padded image) * 5` per file), further bounded
+by half of the free device memory; the patches of a whole group run as one stream of `batch_size` batches that span
+image boundaries (`hvn_infer_tiles`), and equal-size images are post-processed together.  On one GPU a group runs on
+the device while the previous group's files are written and the next group's files are read.  Unlike the reference, a
+file that exceeds the budget on its own is processed as a group of one instead of being skipped."""
 import glob
 import math
 import os
 import pathlib
 import re
 import shutil
+import sys
 
 import numpy as np
 
@@ -119,6 +123,52 @@ def _to_qupath(file_path, nuc_pos_list, nuc_type_list, type_info_dict):
             fptr.write("{x}\t{y}\t{c}\t{n}\t{col}\n".format(x=pos[0], y=pos[1], c="", n=name, col=colour))
 
 
+# Device bytes per image pixel of a tile group (hvn_infer_tiles_dev plus the caller's buffers): packed image 3, map 16,
+# instance map 4, slot-order copies of both when sizes are mixed 20, padded instance table and contour counts
+# 84 / 6 = 14 (each image's table holds min(rows_cap, H*W/6 + 8) rows, whatever the other sizes in the group), packed
+# table and points ~2, post-processing workspace ~95 -- about 155, rounded up.  Per file on top: the 8 extra padded
+# table rows (672 B), the default packed-table and point buffers of a small image (16 rows, 4096 points: 33 KB) and
+# its slot entry.
+DEVICE_BYTES_PER_PX = 192
+DEVICE_BYTES_PER_FILE = 40 << 10
+_END = object()
+
+
+def _padded_shape(h, w, win, step):
+    """Shape of the reflect-padded image `_prepare_patching` builds for an h x w image."""
+    last = lambda length: int((math.ceil((length - step) / step) + 1) * step)  # noqa: E731
+    padt = (win - step) // 2
+    return last(h) + win + padt, last(w) + win + padt, 3
+
+
+def _file_cost(shape, win, step):
+    """(RAM, device) bytes charged for one image of shape [H,W,3]: the reference's `sys.getsizeof(padded image) * 5`
+    (infer/tile.py:271) and DEVICE_BYTES_PER_PX per pixel plus DEVICE_BYTES_PER_FILE."""
+    ram = sys.getsizeof(np.empty(_padded_shape(shape[0], shape[1], win, step), dtype=np.uint8)) * 5
+    return ram, DEVICE_BYTES_PER_PX * int(shape[0]) * int(shape[1]) + DEVICE_BYTES_PER_FILE
+
+
+def _groups(items, costs, budgets):
+    """Cuts the stream `items` into groups, in order (reference infer/tile.py:236-290).  costs(item) -> (ram, device)
+    bytes; budgets() -> (ram, device) bytes, read afresh for every group (device None: no device bound).  A group takes
+    items while their summed costs stay within both budgets (the reference: `available_ram -= expected_usage; if
+    available_ram < 0: break`).  It always takes at least one, so an item over the budget on its own is a group by
+    itself -- the reference drops such a file without processing it."""
+    it = iter(items)
+    nxt = next(it, _END)
+    while nxt is not _END:
+        ram_budget, dev_budget = budgets()
+        group, ram, dev = [], 0, 0
+        while nxt is not _END:
+            r, d = costs(nxt)
+            if group and (ram + r > ram_budget or (dev_budget is not None and dev + d > dev_budget)):
+                break
+            group.append(nxt)
+            ram, dev = ram + r, dev + d
+            nxt = next(it, _END)
+        yield group
+
+
 def _rm_n_mkdir(path):
     if os.path.isdir(path):
         shutil.rmtree(path)
@@ -176,6 +226,56 @@ class InferManager(base.InferManager):
         pred_inst, inst_info_dict = self.post_proc_func(pred_map, nr_types=self.nr_types, return_centroids=True)
         return np.squeeze(pred_map), pred_inst, inst_info_dict
 
+    def infer_images(self, imgs, all_ranks=False):
+        """A group of RGB uint8 images [H_i,W_i,3] -> one (pred_map, pred_inst, inst_info_dict) per image, each equal
+        to `infer_image` on that image alone.
+
+        Device path, one GPU: the patches of all images run as one stream of `batch_size` batches, and equal-size
+        images are post-processed together (`hvn_infer_tiles`).  On several ranks (NCCL) each rank runs its contiguous
+        slice of the group's combined patch list into a zeroed packed map, one NCCL reduce brings the maps to rank 0,
+        and rank 0 post-processes each image (the other ranks get (None, None, None) per image; `all_ranks=True`
+        all_reduces and post-processes everywhere).  Host path: `infer_image` per image."""
+        from ..dist import dist_info, shard_range
+        from ..models.hovernet.post_proc import table_to_dict
+
+        dist, rank, world = dist_info()
+        win = int(self.patch_input_shape)
+        if not (getattr(self, "device_tile_path", False) and (world == 1 or dist.get_backend() == "nccl")):
+            return [self.infer_image(img, all_ranks=all_ranks) for img in imgs]
+        ctx = self.net.ctx
+        if world == 1:
+            return [(np.squeeze(p), i, table_to_dict(t, o, pts, self.nr_types))
+                    for p, i, t, o, pts in ctx.infer_tiles(imgs, win, self.batch_size)]
+        import torch
+        C = ctx.out_shape(win, win)[2]
+        grids = [ctx.tile_grid(img.shape[0], img.shape[1], win) for img in imgs]
+        cells = np.cumsum([0] + [r * c for r, c in grids])
+        px = np.cumsum([0] + [img.shape[0] * img.shape[1] for img in imgs])
+        lo, hi = shard_range(int(cells[-1]), dist.get_rank(), world)
+        d_pred = torch.zeros((int(px[-1]) * C,), dtype=torch.float32, device="cuda")
+        mine = [i for i in range(len(imgs)) if cells[i] < hi and cells[i + 1] > lo]
+        d_imgs = {i: torch.from_numpy(np.ascontiguousarray(imgs[i])).cuda() for i in mine}
+        torch.cuda.synchronize()  # torch's stream -> the library's stream
+        for i in mine:
+            H, W = imgs[i].shape[:2]
+            ctx.tile_predict_dev(d_imgs[i].data_ptr(), H, W, win, max(lo, int(cells[i])) - int(cells[i]),
+                                 min(hi, int(cells[i + 1])) - int(cells[i]), self.batch_size,
+                                 d_pred[int(px[i]) * C:].data_ptr())
+        ctx.sync()
+        if all_ranks:
+            dist.all_reduce(d_pred)
+        else:
+            dist.reduce(d_pred, dst=0)
+            if rank != 0:
+                return [(None, None, None) for _ in imgs]
+        out = []
+        for i, img in enumerate(imgs):
+            H, W = img.shape[:2]
+            m = d_pred[int(px[i]) * C:int(px[i + 1]) * C].view(H, W, C)
+            pred_inst, inst_info_dict = self._post_process_on_device(ctx, m, H, W)
+            out.append((np.squeeze(m.cpu().numpy()), pred_inst, inst_info_dict))
+        return out
+
     def _post_process_on_device(self, ctx, d_pred, H, W):
         """`process` (post_proc.py:94-186) on a device-resident map [H,W,C]: hvn_postproc_dev + hvn_contours_dev, then
         only the instance map, the table rows and the contour points come back.  Same kernels as `post_proc.process`,
@@ -210,9 +310,10 @@ class InferManager(base.InferManager):
         raise RuntimeError("tile post-processing: capacity retries exhausted")
 
     def process_file_list(self, run_args):
-        """Process every image tile under run_args['input_dir'] (reference infer/tile.py:150-388)."""
+        """Process every image tile under run_args['input_dir'] (reference infer/tile.py:150-388), in groups of files
+        (see the module docstring).  On several ranks every file is a group of its own: the ranks must form the same
+        groups, and their free memory differs."""
         import cv2
-        import scipy.io as sio
 
         self.save_qupath = False
         self.save_raw_map = False
@@ -237,16 +338,57 @@ class InferManager(base.InferManager):
         if multi:
             dist.barrier()
 
-        for file_path in file_path_list:
+        win, step = int(self.patch_input_shape), int(self.patch_output_shape)
+        overlap = getattr(self, "device_tile_path", False) and not multi
+        ctx = self.net.ctx if overlap else None
+
+        def read(file_path):
             img = cv2.imread(file_path)
             if img is None:
                 raise IOError("cannot read image %s" % file_path)
-            img = cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
-            img_name = pathlib.Path(file_path).stem
-            pred_map, pred_inst, inst_info_dict = self.infer_image(img)
-            if rank != 0:
-                continue
+            return file_path, cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
 
+        def budgets():
+            if multi:
+                return -1, None
+            import psutil
+            ram = int(psutil.virtual_memory().available * self.mem_usage)
+            # half of the free device memory: the other half stays for the network's activation plans (a new batch
+            # tail builds one, up to ~18 GB for 32 original-mode patches) and the patch batches
+            return ram, (ctx.mem_get_info()[0] // 2 if ctx is not None else None)
+
+        groups = _groups((read(p) for p in file_path_list), lambda f: _file_cost(f[1].shape, win, step), budgets)
+        if not overlap:
+            for files in groups:
+                results = self.infer_images([img for _, img in files])
+                if rank == 0:
+                    self._write_files(files, results)
+            return
+        # one GPU: while group g runs on the device, group g-1's files are written and group g+1's files are read
+        from ..models.hovernet.post_proc import table_to_dict
+        files = next(groups, None)
+        done = None  # (files, results) of the group whose outputs are still to be written
+        while files is not None:
+            job = ctx.infer_tiles_begin([img for _, img in files], win, self.batch_size, want_pred=self.save_raw_map)
+            if done is not None:
+                self._write_files(*done)
+            upcoming = next(groups, None)
+            results = [(None if p is None else np.squeeze(p), i, table_to_dict(t, o, pts, self.nr_types))
+                       for p, i, t, o, pts in job.result()]
+            done = (files, results)
+            files = upcoming
+        if done is not None:
+            self._write_files(*done)
+        return
+
+    def _write_files(self, files, results):
+        """The outputs of one group, file after file: `.mat`, overlay, QuPath TSV and JSON (reference
+        infer/tile.py:326-369)."""
+        import cv2
+        import scipy.io as sio
+
+        for (file_path, img), (pred_map, pred_inst, inst_info_dict) in zip(files, results):
+            img_name = pathlib.Path(file_path).stem
             nuc_val_list = list(inst_info_dict.values())
             nuc_uid_list = np.array(list(inst_info_dict.keys()))[:, None]  # singleton to make matlab happy
             nuc_type_list = np.array([v["type"] for v in nuc_val_list])[:, None]
@@ -266,4 +408,3 @@ class InferManager(base.InferManager):
                 _to_qupath("%s/qupath/%s.tsv" % (self.output_dir, img_name), nuc_coms_list,
                            np.array([v["type"] for v in nuc_val_list]), self.type_info_dict)
             self._save_json("%s/json/%s.json" % (self.output_dir, img_name), inst_info_dict, None)
-        return

@@ -18,6 +18,7 @@
 #ifndef HVN_H_
 #define HVN_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -36,7 +37,7 @@ typedef enum {
     HVN_ERR_RANGE = -6        /* an activation left the representable range of the engine's fp16 hi+lo storage
                                  (|x| > 65504 * 2^act_shift); outputs of that call are invalid.  Raise option
                                  "act_shift" (exact power-of-two rescaling of all activations) and run again.  Reported
-                                 by the call that synchronises: hvn_forward / hvn_forward_postproc / hvn_infer_tile,
+                                 by the call that synchronises: hvn_forward / hvn_forward_postproc / hvn_infer_tile(s),
                                  or, after *_dev calls, hvn_sync / hvn_timer_stop. */
 } hvn_status;
 
@@ -91,7 +92,9 @@ int hvn_finalize_weights(hvn_ctx *ctx);
  *                      fp32-accumulation noise (tests/test_cnn_gpu.py::test_kernel_variants_agree). */
 int hvn_set_option(hvn_ctx *ctx, const char *key, int64_t value);
 const char *hvn_debug_log(const hvn_ctx *ctx);
-/* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing and contour kernels), "last_flops" (algorithmic 2*MACs of the
+/* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing and contour kernels), "tile_table_rows" (rows
+ * of padded instance tables the last hvn_infer_tiles* group of two or more images held in the context's workspace:
+ * min(rows_cap, H*W/6 + 8) per image, 84 B each), "last_flops" (algorithmic 2*MACs of the
  * last forward), "precision" (0 | 1), "plan_bytes" (device bytes of the activation buffers of the plan(s) the last
  * forward ran); with option "profile" = 2 also "launches:<class>" and "flops:<class>" for
  * class in {conv_tc, conv_ref, conv0, bnrelu, head} (see hvn_stage_ms). */
@@ -153,6 +156,32 @@ int hvn_infer_tile(hvn_ctx *ctx, const uint8_t *img_host, int H, int W, int patc
                    int32_t *inst_host, int64_t *table_host, int max_rows, int32_t *n_rows_host, int32_t *pts_host,
                    int64_t pts_cap, int32_t *offs_host);
 
+/* ---- tile path over a group of images (reference infer/tile.py:236-369, which runs the patches of every cached file
+ * as one stream of batches): n_images >= 1 images of any sizes, shapes [n_images][2] = (H, W) (a host array in both
+ * variants), images u8 [H_i,W_i,3] packed back to back in input order.  All patches form one list, image after image,
+ * cut into batches of `batch` (0 = default) that may span two or more images; each image's result is bit-identical to
+ * hvn_infer_tile on that image alone.  Outputs, all in input order:
+ *   pred [H_i,W_i,C] back to back (may be NULL), inst [H_i,W_i] back to back;
+ *   table [rows_cap,10]: the instance rows of image i are table[row_offs[i] : row_offs[i+1]], row_offs [n_images+1];
+ *   contours when pt_offs is not NULL: pt_offs [rows_cap+1], the points of packed row r are
+ *   pts[pt_offs[r] : pt_offs[r+1]] (pts [pts_cap,2] (x, y); entries past row_offs[n_images] repeat the total).
+ * Images of equal size are post-processed together, one call per size.  HVN_ERR_CAPACITY when row_offs[n_images] >
+ * rows_cap (row_offs is valid then) or, the table fitting, when the points exceed pts_cap (pt_offs is valid then): size
+ * the buffers from the offsets and call again.  HVN_ERR_INVALID on n_images < 1, a bad shape or rows_cap < 1.
+ *   hvn_infer_tiles     : host buffers; synchronises, reports HVN_ERR_RANGE.
+ *   hvn_infer_tiles_dev : device buffers (shapes stays on the host), stream-ordered on the context stream with no host
+ *                         synchronisation, so the caller can overlap host work; the offsets are read (and range and
+ *                         capacity checked) after hvn_sync, as for hvn_contours_dev.  Device workspace (context-owned,
+ *                         grow-only): the padded instance tables of the group (min(rows_cap, H_i*W_i/6 + 8) rows of
+ *                         84 B per image, counter "tile_table_rows"), and the maps in size order when that differs
+ *                         from the input order. */
+int hvn_infer_tiles(hvn_ctx *ctx, int n_images, const uint8_t *imgs_host, const int32_t *shapes, int patch_in,
+                    int batch, float *pred_host, int32_t *inst_host, int64_t *table_host, int64_t rows_cap,
+                    int32_t *row_offs_host, int32_t *pts_host, int64_t pts_cap, int32_t *pt_offs_host);
+int hvn_infer_tiles_dev(hvn_ctx *ctx, int n_images, const uint8_t *imgs_dev, const int32_t *shapes, int patch_in,
+                        int batch, float *pred_dev, int32_t *inst_dev, int64_t *table_dev, int64_t rows_cap,
+                        int32_t *row_offs_dev, int32_t *pts_dev, int64_t pts_cap, int32_t *pt_offs_dev);
+
 /* ---- end-of-batch gather support (SURVEY.md 8e; replaces the reference's DataParallel gather, infer/base.py:69):
  * hvn_pack_tables_dev compacts the padded tables of a batch, table_dev [n_maps,max_rows,10] + n_rows_dev [n_maps],
  * into packed_dev [<= cap_rows,10] (map order, no padding) and offs_dev [n_maps + 1] int32 (row range of map m =
@@ -213,6 +242,8 @@ int hvn_free_host(hvn_ctx *ctx, void *host_ptr);
 int hvn_memcpy_h2d(hvn_ctx *ctx, void *dst_dev, const void *src_host, size_t bytes);
 int hvn_memcpy_d2h(hvn_ctx *ctx, void *dst_host, const void *src_dev, size_t bytes);
 int hvn_sync(hvn_ctx *ctx);
+/* cudaMemGetInfo on the context's device: free and total bytes (e.g. to size a tile group). */
+int hvn_mem_info(hvn_ctx *ctx, size_t *free_bytes, size_t *total_bytes);
 /* CUDA-event timing on the context stream (the stream every kernel of this library is launched
  * on): hvn_timer_start .. hvn_timer_stop returns elapsed milliseconds. */
 int hvn_timer_start(hvn_ctx *ctx);
