@@ -133,71 +133,14 @@ __device__ __forceinline__ void conv_epilogue4(const ConvParams &P, int n, int o
     }
 }
 
-
-// ---- two-phase form: issue the (independent) global loads of several
-// output pixels first, then finish them, so that the residual / skip read latency overlaps.
+// Epilogue variants of the wgmma kernel (k_conv_tc's MODE): plain, + residual, 2x upsample + skip.
 enum { EPI_PLAIN = 0, EPI_RES = 1, EPI_UP2 = 2 };
-
-template <int MODE> struct EpiPre;
-template <> struct EpiPre<EPI_PLAIN> {};
-template <> struct EpiPre<EPI_RES> { float4 r; };
-template <> struct EpiPre<EPI_UP2> { uint2 h[4], l[4]; };
-
-template <int MODE>
-__device__ __forceinline__ void epi_prefetch(const ConvParams &P, int n, int oy, int ox, int c, EpiPre<MODE> &pre) {
-    if constexpr (MODE == EPI_RES) {
-        pre.r = *reinterpret_cast<const float4 *>(P.res.p + n * P.res.sN + (long long)oy * P.res.sH +
-                                                  (long long)ox * P.res.sW + c);
-    } else if constexpr (MODE == EPI_UP2) {
-#pragma unroll
-        for (int d = 0; d < 4; ++d) {
-            int Y = 2 * oy + (d >> 1), X = 2 * ox + (d & 1);
-            long long so = n * P.skip.sN + (long long)Y * P.skip.sH + (long long)X * P.skip.sW + c;
-            pre.h[d] = *reinterpret_cast<const uint2 *>(P.skip.hi + so);
-            pre.l[d] = P.skip.lo ? *reinterpret_cast<const uint2 *>(P.skip.lo + so) : make_uint2(0u, 0u);
-        }
-    }
-}
 
 __device__ __forceinline__ void store_split4(const SplitRef &o, long long off, const float t[4]) {
     uint2 oh, ol;
     split4_f32(t, oh, ol, o.flag);
     *reinterpret_cast<uint2 *>(o.hi + off) = oh;
     if (o.lo) *reinterpret_cast<uint2 *>(o.lo + off) = ol;
-}
-
-// sc / sh: the BN scale / shift of channels c..c+3, loaded once per tile by the caller (they do not depend
-// on the pixel; loading them per store left the write-out loop waiting on global loads).
-// ws: 2^-e of the four channels (ConvWeights::oscale), applied to the accumulator first.
-template <int MODE>
-__device__ __forceinline__ void epi_finish(const ConvParams &P, int n, int oy, int ox, int c, float v[4],
-                                           const EpiPre<MODE> &pre, const float4 &s, const float4 &b, const float4 &ws) {
-    v[0] *= ws.x; v[1] *= ws.y; v[2] *= ws.z; v[3] *= ws.w;
-    if constexpr (MODE == EPI_RES) { v[0] += pre.r.x; v[1] += pre.r.y; v[2] += pre.r.z; v[3] += pre.r.w; }
-    if (P.out_raw.p) {
-        float *o = P.out_raw.p + n * P.out_raw.sN + (long long)oy * P.out_raw.sH + (long long)ox * P.out_raw.sW + c;
-        *reinterpret_cast<float4 *>(o) = make_float4(v[0], v[1], v[2], v[3]);
-    }
-    if constexpr (MODE == EPI_UP2) {
-#pragma unroll
-        for (int d = 0; d < 4; ++d) {
-            int Y = 2 * oy + (d >> 1), X = 2 * ox + (d & 1);
-            const __half *hh = reinterpret_cast<const __half *>(&pre.h[d]);
-            const __half *ll = reinterpret_cast<const __half *>(&pre.l[d]);
-            float t[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) t[i] = v[i] + join_f16(hh[i], ll[i]);
-            store_split4(P.out_split, n * P.out_split.sN + (long long)Y * P.out_split.sH + (long long)X * P.out_split.sW + c, t);
-        }
-    } else if (P.out_split.hi) {
-        float t[4] = {v[0], v[1], v[2], v[3]};
-        if (P.scale) { t[0] = t[0] * s.x + b.x; t[1] = t[1] * s.y + b.y; t[2] = t[2] * s.z + b.z; t[3] = t[3] * s.w + b.w; }
-        if (P.relu) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) t[i] = fmaxf(t[i], 0.f);
-        }
-        store_split4(P.out_split, n * P.out_split.sN + (long long)oy * P.out_split.sH + (long long)ox * P.out_split.sW + c, t);
-    }
 }
 
 }  // namespace hvn

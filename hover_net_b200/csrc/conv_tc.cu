@@ -32,6 +32,7 @@
 #include <algorithm>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "conv_epilogue.cuh"
@@ -102,41 +103,60 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, fp32 accumulators in registers.
 // Fragment: register 4j + 2h + e holds row (warp & 3) * 16 + lane / 4 + 8h, column 8j + 2 (lane % 4) + e.
+// mma: D = A*B + (accum ? D : 0).  mma0: D = A*B with D write-only (scale-d = false), so the accumulator's previous
+// contents are dead for the compiler too and its registers are free between a drain and the next segment's first MMA.
 template <int N> struct Wgmma;
-#define HVN_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-#define HVN_WGMMA(N, R, DREGS, P, AB, ...)                                                                             \
+#define HVN_F8(M, i) M(d[i]), M(d[i + 1]), M(d[i + 2]), M(d[i + 3]), M(d[i + 4]), M(d[i + 5]), M(d[i + 6]), M(d[i + 7])
+#define HVN_D16(M) HVN_F8(M, 0), HVN_F8(M, 8)
+#define HVN_D32(M) HVN_D16(M), HVN_F8(M, 16), HVN_F8(M, 24)
+#define HVN_D64(M) HVN_D32(M), HVN_F8(M, 32), HVN_F8(M, 40), HVN_F8(M, 48), HVN_F8(M, 56)
+#define HVN_WGMMA(N, R, DREGS, P, AB, DCONS)                                                                           \
     template <> struct Wgmma<N> {                                                                                      \
         static __device__ __forceinline__ void mma(float (&d)[R], uint64_t a, uint64_t b, uint32_t accum) {            \
             asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\twgmma.mma_async.sync.aligned.m64n" #N      \
                          "k16.f32.f16.f16 {" DREGS "}, " AB ", p, 1, 1, 0, 0;\n\t}"                                    \
-                         : __VA_ARGS__ : "l"(a), "l"(b), "r"(accum));                                                  \
+                         : DCONS("+f") : "l"(a), "l"(b), "r"(accum));                                                  \
+        }                                                                                                              \
+        static __device__ __forceinline__ void mma0(float (&d)[R], uint64_t a, uint64_t b) {                           \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 0, 0;\n\twgmma.mma_async.sync.aligned.m64n" #N          \
+                         "k16.f32.f16.f16 {" DREGS "}, " AB ", p, 1, 1, 0, 0;\n\t}"                                    \
+                         : DCONS("=f") : "l"(a), "l"(b));                                                              \
         }                                                                                                              \
     };
-HVN_WGMMA(32, 16, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15", "%18", "%16, %17", HVN_F8(0), HVN_F8(8))
-HVN_WGMMA(64, 32, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31", "%34", "%32, %33", HVN_F8(0), HVN_F8(8), HVN_F8(16), HVN_F8(24))
-HVN_WGMMA(128, 64, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63", "%66", "%64, %65", HVN_F8(0), HVN_F8(8), HVN_F8(16), HVN_F8(24), HVN_F8(32), HVN_F8(40), HVN_F8(48), HVN_F8(56))
+HVN_WGMMA(32, 16, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15", "%18", "%16, %17", HVN_D16)
+HVN_WGMMA(64, 32, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31", "%34", "%32, %33", HVN_D32)
+HVN_WGMMA(128, 64, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63", "%66", "%64, %65", HVN_D64)
 #undef HVN_WGMMA
+#undef HVN_D64
+#undef HVN_D32
+#undef HVN_D16
 #undef HVN_F8
 
-// One 64-channel K-slice of the split product: a_hi*w_hi + a_hi*w_lo + a_lo*w_hi (4 K=16 steps, +32 B each)
-template <int N>
-__device__ __forceinline__ void mma_slice(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, bool zero) {
+// One 64-channel K-slice of the split product: a_hi*w_hi + a_hi*w_lo + a_lo*w_hi (4 K=16 steps, +32 B each).
+// ZERO: the slice starts a segment, its first MMA overwrites the accumulator (write-only); zero: the same at run time.
+template <int N, bool ZERO = false>
+__device__ __forceinline__ void mma_slice(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                          bool zero = false) {
     const uint64_t dah = wg_desc(a_hi), dal = wg_desc(a_lo), dbh = wg_desc(b_hi), dbl = wg_desc(b_lo);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const uint64_t ko = (uint64_t)(2 * k);
-        Wgmma<N>::mma(d, dah + ko, dbh + ko, (zero && k == 0) ? 0u : 1u);
+        if (ZERO && k == 0) Wgmma<N>::mma0(d, dah + ko, dbh + ko);
+        else Wgmma<N>::mma(d, dah + ko, dbh + ko, (zero && k == 0) ? 0u : 1u);
         Wgmma<N>::mma(d, dah + ko, dbl + ko, 1u);
         Wgmma<N>::mma(d, dal + ko, dbh + ko, 1u);
     }
 }
 
 // One 64-channel K-slice of the single product a_hi*w_hi (precision "high")
-template <int N>
-__device__ __forceinline__ void mma_slice1(float (&d)[N / 2], uint32_t a_hi, uint32_t b_hi, bool zero) {
+template <int N, bool ZERO = false>
+__device__ __forceinline__ void mma_slice1(float (&d)[N / 2], uint32_t a_hi, uint32_t b_hi, bool zero = false) {
     const uint64_t dah = wg_desc(a_hi), dbh = wg_desc(b_hi);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) Wgmma<N>::mma(d, dah + 2 * k, dbh + 2 * k, (zero && k == 0) ? 0u : 1u);
+    for (int k = 0; k < 4; ++k) {
+        if (ZERO && k == 0) Wgmma<N>::mma0(d, dah, dbh);
+        else Wgmma<N>::mma(d, dah + 2 * k, dbh + 2 * k, (zero && k == 0) ? 0u : 1u);
+    }
 }
 
 struct TcGeom {
@@ -204,25 +224,30 @@ __device__ __forceinline__ void store_split2(const SplitRef &o, long long off, f
     *reinterpret_cast<__half2 *>(o.lo + off) = __halves2half2(l0, l1);
 }
 
-// Channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  Same operations, in the same order, as
-// epi_finish (conv_epilogue.cuh) on four channels.
+// fp16 pairs parked in fp32 registers (the epilogue's skip batch lives in the dead accumulator)
+__device__ __forceinline__ float ld_bits(const __half *p) { return __uint_as_float(*reinterpret_cast<const uint32_t *>(p)); }
+__device__ __forceinline__ __half2 bits_h2(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return *reinterpret_cast<const __half2 *>(&u);
+}
+
+// Channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  The global reads were issued earlier into
+// `pre`: EPI_RES the residual pair {r.x, r.y}; EPI_UP2 the skip pairs of the four output pixels, hi (and, unless ONE,
+// lo) as fp16x2 bits, [d * planes + plane].
 template <int MODE, bool ONE>
-__device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, float2 s, float2 b) {
-    if constexpr (MODE == EPI_RES) {
-        const float2 r = *reinterpret_cast<const float2 *>(P.res.p + o.res + c);
-        v0 += r.x; v1 += r.y;
-    }
+__device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, float2 s, float2 b,
+                                            const float *pre) {
+    if constexpr (MODE == EPI_RES) { v0 += pre[0]; v1 += pre[1]; }
     if (o.raw >= 0) *reinterpret_cast<float2 *>(P.out_raw.p + o.raw + c) = make_float2(v0, v1);
     if constexpr (MODE == EPI_UP2) {
 #pragma unroll
         for (int d = 0; d < 4; ++d) {
-            const long long so = o.skip + (d >> 1) * P.skip.sH + (d & 1) * P.skip.sW + c;
-            const __half2 sh = *reinterpret_cast<const __half2 *>(P.skip.hi + so);
             const long long oo = o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c;
             if constexpr (ONE) {
+                const __half2 sh = bits_h2(pre[d]);
                 store_split2<true>(P.out_split, oo, v0 + __half2float(sh.x), v1 + __half2float(sh.y));
             } else {
-                const __half2 sl = *reinterpret_cast<const __half2 *>(P.skip.lo + so);
+                const __half2 sh = bits_h2(pre[2 * d]), sl = bits_h2(pre[2 * d + 1]);
                 store_split2<false>(P.out_split, oo, v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
             }
         }
@@ -457,31 +482,43 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
             const int tm = tile / G.tiles_n, tn = tile - tm * G.tiles_n;
 #pragma unroll
             for (int j = 0; j < NR; ++j) sum[j] = 0.f;
-            int pend = -1;   // stage whose wgmma group may still be reading it
-            for (int it = 0; it < kiters; ++it, ++it_global) {
+            // Segments of G.seg K-slices.  Inside one, a slice's wgmma group is issued before the previous slice's group
+            // is waited for, so one group is always in flight; only the segment's end waits for all of them and drains
+            // the accumulator into the fp32 sum.  Every exit of the inner loop reaches that wait, and the segment's first
+            // MMA does not read the accumulator, so ptxas needs to inject no wait of its own; the register fences keep
+            // the accumulator untouched around the asynchronous MMAs.
+            int pend;   // stage whose wgmma group may still be reading it
+            auto slice = [&](auto zero) {
                 const int s = it_global % STAGES;
                 mbar_wait(full_bar(s), (uint32_t)(it_global / STAGES) & 1u);
                 const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;
                 const uint32_t sb = smem_base + s * STAGE_BYTES + PLANES * A_TILE_BYTES;
+                wg_fence_regs(acc);
                 wg_fence();
-                if constexpr (ONE) mma_slice1<BLOCK_N>(acc, sa, sb, it % G.seg == 0);
-                else mma_slice<BLOCK_N>(acc, sa, sa + A_TILE_BYTES, sb, sb + BLOCK_N * 128, it % G.seg == 0);
+                if constexpr (ONE) mma_slice1<BLOCK_N, decltype(zero)::value>(acc, sa, sb);
+                else mma_slice<BLOCK_N, decltype(zero)::value>(acc, sa, sa + A_TILE_BYTES, sb, sb + BLOCK_N * 128);
                 wg_commit();
-                if ((it + 1) % G.seg == 0 || it + 1 == kiters) {   // segment complete: drain it into the fp32 sum
-                    wg_wait<0>();
-                    wg_fence_regs(acc);
-                    if (pend >= 0) release(pend);
-                    release(s);
-                    pend = -1;
+                wg_fence_regs(acc);
+                wg_wait<1>();                                      // the previous slice's group is done with its stage
+                if (pend >= 0) release(pend);
+                pend = s;
+                ++it_global;
+            };
+            for (int it0 = 0; it0 < kiters; it0 += G.seg) {
+                const int it1 = min(it0 + G.seg, kiters);
+                pend = -1;
+                slice(std::true_type{});
+                for (int it = it0 + 1; it < it1; ++it) slice(std::false_type{});
+                wg_wait<0>();                                      // segment complete: drain it into the fp32 sum
+                wg_fence_regs(acc);
+                release(pend);
 #pragma unroll
-                    for (int j = 0; j < NR; ++j) sum[j] += acc[j];
-                } else {
-                    wg_wait<1>();                                  // the previous slice's group is done with its stage
-                    if (pend >= 0) release(pend);
-                    pend = s;
-                }
+                for (int j = 0; j < NR; ++j) sum[j] += acc[j];
             }
-            // ---- epilogue straight from the fragment: rows ra, ra + 8; two consecutive channels per register pair
+            // ---- epilogue straight from the fragment: rows ra, ra + 8; two consecutive channels per register pair.
+            // acc is dead until the next tile's first wgmma (scale-d = 0), so it holds what the epilogue reads from global
+            // memory: all of a batch's reads are issued before its first store.  The compiler cannot hoist them itself,
+            // since res may alias out_raw and skip may alias out_split.
             PixOff po[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -507,16 +544,57 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 po[h] = pix_offsets<MODE>(P, valid, n_img, oy, ox);
             }
             const bool bn = MODE != EPI_UP2 && P.scale && P.out_split.hi;
+            // EPI_RES: the whole fragment's residual, one float2 per register pair (one round trip per tile)
+            if constexpr (MODE == EPI_RES) {
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) {
-                const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
-                const float2 ws = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
-                float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
-                if (bn) { sc = __ldg(reinterpret_cast<const float2 *>(P.scale + c)); sh = __ldg(reinterpret_cast<const float2 *>(P.shift + c)); }
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (po[h].raw >= 0 || po[h].spl >= 0)
-                        epi_finish2<MODE, ONE>(P, po[h], c, sum[4 * j + 2 * h] * ws.x, sum[4 * j + 2 * h + 1] * ws.y, sc, sh);
+                    for (int h = 0; h < 2; ++h)
+                        if (po[h].res >= 0) {
+                            const float2 r = *reinterpret_cast<const float2 *>(P.res.p + po[h].res + c);
+                            acc[4 * j + 2 * h] = r.x; acc[4 * j + 2 * h + 1] = r.y;
+                        }
+                }
+            }
+            // Batches of JB column groups j, their per-channel scales loaded up front.  EPI_UP2: the skip pairs of a batch
+            // (2 rows x 4 output pixels x planes per j) go into acc, four round trips per tile.  The batch sizes are the
+            // largest that stay within 168 registers without spilling at BLOCK_N = 128.
+            constexpr int JB = MODE == EPI_UP2 ? NR / 16 : 2;
+            static_assert((BLOCK_N / 8) % JB == 0, "epilogue batch must divide the column groups");
+#pragma unroll
+            for (int j0 = 0; j0 < BLOCK_N / 8; j0 += JB) {
+                float2 ws[JB], sc[JB], sh[JB];
+#pragma unroll
+                for (int jj = 0; jj < JB; ++jj) {
+                    const int c = tn * BLOCK_N + 8 * (j0 + jj) + 2 * (lane & 3);
+                    ws[jj] = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
+                    sc[jj] = make_float2(1.f, 1.f); sh[jj] = make_float2(0.f, 0.f);
+                    if (bn) { sc[jj] = __ldg(reinterpret_cast<const float2 *>(P.scale + c)); sh[jj] = __ldg(reinterpret_cast<const float2 *>(P.shift + c)); }
+                    if constexpr (MODE == EPI_UP2) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            if (po[h].skip >= 0)
+#pragma unroll
+                                for (int d = 0; d < 4; ++d) {
+                                    const long long so = po[h].skip + (d >> 1) * P.skip.sH + (d & 1) * P.skip.sW + c;
+                                    float *pre = &acc[((jj * 2 + h) * 4 + d) * PLANES];
+                                    pre[0] = ld_bits(P.skip.hi + so);
+                                    if constexpr (!ONE) pre[1] = ld_bits(P.skip.lo + so);
+                                }
+                    }
+                }
+#pragma unroll
+                for (int jj = 0; jj < JB; ++jj) {
+                    const int j = j0 + jj;
+                    const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        if (po[h].raw >= 0 || po[h].spl >= 0)
+                            epi_finish2<MODE, ONE>(P, po[h], c, sum[4 * j + 2 * h] * ws[jj].x, sum[4 * j + 2 * h + 1] * ws[jj].y,
+                                                   sc[jj], sh[jj],
+                                                   MODE == EPI_UP2 ? &acc[(jj * 2 + h) * 4 * PLANES] : &acc[4 * j + 2 * h]);
+                }
             }
         }
     }

@@ -11,15 +11,17 @@ def classify(name, k, stride, cin, cout, out, bn, halo):
         if cout >= 128:
             return "wide kxk (cout >= 128)"
         return "thin kxk (cout 64)"
-    if ".dense.units." in name or name.endswith("convf.weight"):
-        return "1x1 XF decoder (dense conv1, convf)"
+    if name.startswith("conv_bot") or name.endswith("convf.weight"):
+        return "1x1 + upsample/skip (conv_bot, convf)"
+    if ".dense.units." in name:
+        return "1x1 XF decoder (dense conv1)"
     if "conv1" in name and ".units.0." not in name:
         return "1x1 XF encoder (pre-activation conv1)"
     if "conv3" in name and "shortcut" not in name:
         return "1x1 + residual (conv3, d0 at full resolution)" if name.startswith("d0.") else "1x1 + residual (conv3, d1-d3)"
     if name.startswith("d0."):
         return "1x1 plain, d0 (full resolution)"
-    return "1x1 plain (unit-0 conv1, conv3+shortcut, conv_bot)"
+    return "1x1 plain (unit-0 conv1, conv3+shortcut)"
 
 
 def main(path):
