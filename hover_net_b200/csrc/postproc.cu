@@ -475,15 +475,18 @@ __global__ void k_range_init(int2 *r, size_t n) {
 // and exactly by one thread with a private binary heap (same sift rules as heap_general.pxi).
 struct __align__(16) HeapItem { double v; int age; int idx; };
 
+// (value, age), then raster index: only age-0 marker pixels can tie on (value, age), and they pop in raster order as in
+// the shared-memory floods (DESIGN.md 2)
 __device__ __forceinline__ bool h_smaller(const HeapItem &a, const HeapItem &b) {
     if (a.v != b.v) return a.v < b.v;
-    return a.age < b.age;
+    if (a.age != b.age) return a.age < b.age;
+    return a.idx < b.idx;
 }
 
-// 4-ary min-heap on (value, age): the first WS_CAP entries (the hot top levels) live in shared memory,
-// the rest in the blob's slice of the global arena.  Keys are a strict total order (apart from
-// equal-valued marker pixels, see DESIGN.md), so the pop sequence -- all that the flood depends on --
-// is the same as for skimage's binary heap.
+// 4-ary min-heap on (value, age, idx): the first WS_CAP entries (the hot top levels) live in shared memory,
+// the rest in the blob's slice of the global arena.  Keys are a strict total order, so the pop sequence -- all
+// that the flood depends on -- is the same as for skimage's binary heap (apart from equal-valued marker pixels,
+// which skimage pops in heap-layout order, see DESIGN.md).
 constexpr int WS_CAP = 2048;
 struct Heap4 {
     HeapItem *s, *g;
@@ -694,7 +697,10 @@ k_watershed_tile(int H, int W, int big_cap, const double *__restrict__ dist_all,
                  HeapItem *__restrict__ heap_all, int *__restrict__ inst_all, PPStats *st) {
     extern __shared__ __align__(16) unsigned char wt_smem[];
     __shared__ int s_next[2];
-    const unsigned int wmagic = (unsigned int)((0x100000000ull + (unsigned)W - 1) / (unsigned)W);  // idx / W for idx < 2^16
+    // y = idx / W for idx < 2^16 as umulhi(idx, ceil(2^32 / W)) + (idx & wone); for W = 1 the multiplier (2^32) does not
+    // fit in 32 bits, so it is 0 there and wone = ~0 passes idx through.
+    const unsigned int wmagic = W > 1 ? (unsigned int)((0x100000000ull + (unsigned)W - 1) / (unsigned)W) : 0u;
+    const unsigned int wone = W > 1 ? 0u : 0xffffffffu;
     const int m = blockIdx.x, N = H * W;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // layout: heaps (u64, 16-byte aligned groups) | kk (float per px, optional) | state (int16 per px)
@@ -768,7 +774,7 @@ k_watershed_tile(int H, int W, int big_cap, const double *__restrict__ dist_all,
                 const u64 e = hp.pop();
                 ++npop;
                 const int idx = (int)((unsigned int)e & 0xffffu);
-                const int y = (int)__umulhi((unsigned int)idx, wmagic), x = idx - y * W;
+                const int y = (int)(__umulhi((unsigned int)idx, wmagic) + ((unsigned int)idx & wone)), x = idx - y * W;
                 const short lab = state[idx];
                 const int q[4] = {y > 0 ? idx - W : -1, x > 0 ? idx - 1 : -1, x < W - 1 ? idx + 1 : -1, y < H - 1 ? idx + W : -1};
                 bool take[4];
@@ -818,7 +824,8 @@ k_watershed_cal(int H, int W, const double *__restrict__ dist_all, const unsigne
     extern __shared__ __align__(16) unsigned char wc_smem[];
     __shared__ int s_next[2];
     __shared__ unsigned int s_kmin, s_kmax;
-    const unsigned int wmagic = (unsigned int)((0x100000000ull + (unsigned)W - 1) / (unsigned)W);
+    const unsigned int wmagic = W > 1 ? (unsigned int)((0x100000000ull + (unsigned)W - 1) / (unsigned)W) : 0u;  // as in
+    const unsigned int wone = W > 1 ? 0u : 0xffffffffu;                                                       // k_watershed_tile
     const int m = blockIdx.x, N = H * W;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const size_t n8 = ((size_t)N * 8 + 15) & ~(size_t)15;
@@ -944,7 +951,7 @@ k_watershed_cal(int H, int W, const double *__restrict__ dist_all, const unsigne
                     if (!w2) summary &= ~(1ull << j);
                 }
                 ++npop;
-                const int y = (int)__umulhi((unsigned int)idx, wmagic), x = idx - y * W;
+                const int y = (int)(__umulhi((unsigned int)idx, wmagic) + ((unsigned int)idx & wone)), x = idx - y * W;
                 const short lab = e.state;
                 const int q[4] = {y > 0 ? idx - W : -1, x > 0 ? idx - 1 : -1, x < W - 1 ? idx + 1 : -1, y < H - 1 ? idx + W : -1};
                 PxRec nr[4];
@@ -1053,6 +1060,84 @@ __global__ void k_table_rows(const InstAcc *__restrict__ acc_all, const int *__r
 static int g_flood_impl = 0;  // 0 auto (calendar queue > shared-memory heap > global heap), 1 no calendar queue, 2 global only
 void postproc_set_flood_impl(int v) { g_flood_impl = v; }
 
+const char *postproc_flood_name(int k) {
+    switch (k) {
+    case FLOOD_CAL: return "k_watershed_cal";
+    case FLOOD_TILE_KK: return "k_watershed_tile<true>";
+    case FLOOD_TILE: return "k_watershed_tile<false>";
+    case FLOOD_GLOBAL: return "k_watershed";
+    default: return "?";
+    }
+}
+
+// Shared-memory plan of the per-map flood kernels for an N-px map.  The calendar queue holds one 8-byte record per
+// pixel; the heap kernel holds the int16 flood state, optionally the fp32 key table (kk), the small-blob heaps and
+// a large-blob heap of `cap` entries (capped at 16384, at least 1024 for the kernel to be worth running).
+struct FloodPlan {
+    size_t cal_bytes, tile_smem[2];  // tile_smem[kk]
+    long long cap[2];
+    bool cal_ok, tile_ok[2];
+};
+static const size_t kFloodBudget = 225 * 1024;
+
+static FloodPlan flood_plan(int N, int max_ids) {
+    FloodPlan f;
+    const size_t state_bytes = (((size_t)N * 2 + 15) & ~(size_t)15), kk_bytes = (((size_t)N * 4 + 15) & ~(size_t)15);
+    f.cal_bytes = (((size_t)N * 8 + 15) & ~(size_t)15) + 2 * (WC_NB_BIG * 2 + WC_NB_BIG / 8) +
+                  (WT_WARPS - 2) * (WC_NB_SMALL * 2 + WC_NB_SMALL / 8);
+    f.cal_ok = f.cal_bytes <= kFloodBudget && N < 65535 && max_ids < 32000;
+    const size_t small_bytes = (size_t)(WT_WARPS - 1) * (WT_SMALL_CAP + 4) * 8;
+    for (int kk = 0; kk < 2; ++kk) {
+        const size_t fixed = state_bytes + (kk ? kk_bytes : 0) + small_bytes;
+        long long cap = fixed + 64 < kFloodBudget ? (long long)((kFloodBudget - fixed) / 8) - 4 : 0;
+        cap = std::min<long long>(cap & ~3ll, 16384);
+        f.cap[kk] = cap;
+        f.tile_smem[kk] = fixed + (size_t)(cap + 4) * 8;
+        f.tile_ok[kk] = cap >= 1024 && N < 65536 && max_ids < 32000;
+    }
+    // the key table is used whenever it leaves room for a 2048-entry large heap
+    f.tile_ok[1] = f.tile_ok[1] && state_bytes + kk_bytes + small_bytes + (2048 + 4) * 8 <= kFloodBudget;
+    return f;
+}
+
+int postproc_flood(cudaStream_t stream, const PostprocBuffers &b, int n, int H, int W, int *inst, int choice) {
+    const int N = H * W;
+    const FloodPlan f = flood_plan(N, b.max_ids);
+    int k = choice;
+    if (k == FLOOD_AUTO) {  // patch-sized maps: per-map CTA with the flood state in shared memory; otherwise the generic kernel
+        if (f.cal_ok && g_flood_impl == 0) k = FLOOD_CAL;
+        else if (f.tile_ok[0] && g_flood_impl <= 1) k = f.tile_ok[1] ? FLOOD_TILE_KK : FLOOD_TILE;
+        else k = FLOOD_GLOBAL;
+    }
+    HVN_CHECK(k >= FLOOD_CAL && k <= FLOOD_GLOBAL, -1, "postproc_flood: unknown flood kernel");
+    HVN_CHECK(k != FLOOD_CAL || f.cal_ok, -1, "postproc_flood: the calendar-queue flood does not fit this map");
+    HVN_CHECK(k != FLOOD_TILE_KK || f.tile_ok[1], -1, "postproc_flood: the heap flood with key table does not fit this map");
+    HVN_CHECK(k != FLOOD_TILE || f.tile_ok[0], -1, "postproc_flood: the shared-memory heap flood does not fit this map");
+    static bool attr = false;
+    if (!attr) {
+        HVN_CUDA(cudaFuncSetAttribute(k_watershed_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFloodBudget + 64));
+        HVN_CUDA(cudaFuncSetAttribute(k_watershed_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFloodBudget + 64));
+        HVN_CUDA(cudaFuncSetAttribute(k_watershed_cal, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFloodBudget + 64));
+        attr = true;
+    }
+    PPStats *st = (PPStats *)b.stats;
+    if (k == FLOOD_CAL) {
+        k_watershed_cal<<<n, WT_WARPS * 32, f.cal_bytes, stream>>>(H, W, b.dist, b.fg, b.L1, b.size1, b.blob_root, (int4 *)b.bbox,
+                                                                 (const int2 *)b.lab_range, b.max_blobs, inst, st);
+    } else if (k == FLOOD_TILE_KK) {
+        k_watershed_tile<true><<<n, WT_WARPS * 32, f.tile_smem[1], stream>>>(H, W, (int)f.cap[1], b.dist, b.fg, b.L1, b.size1,
+            b.blob_root, (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs, (HeapItem *)b.heap, inst, st);
+    } else if (k == FLOOD_TILE) {
+        k_watershed_tile<false><<<n, WT_WARPS * 32, f.tile_smem[0], stream>>>(H, W, (int)f.cap[0], b.dist, b.fg, b.L1, b.size1,
+            b.blob_root, (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs, (HeapItem *)b.heap, inst, st);
+    } else {
+        k_watershed<<<dim3((unsigned)b.max_blobs, (unsigned)n), 32, WS_CAP * sizeof(HeapItem), stream>>>(
+            H, W, b.dist, b.fg, b.L1, b.size1, b.blob_root, (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs,
+            (HeapItem *)b.heap, inst, st);
+    }
+    return k;
+}
+
 template <typename A>
 static void pp_layout(A &ar, PostprocBuffers &b, int n, int H, int W, int nr_types) {
     size_t N = (size_t)H * W, T = (size_t)n * N;
@@ -1160,39 +1245,9 @@ int postproc_run(Arena &arena, cudaStream_t stream, const float *pred, int n, in
     L(k_blob_marker_range<<<g1, TPB, 0, stream>>>(N, inst, b.L1, b.blob_of_root, (int2 *)b.lab_range, b.max_blobs));
     L(k_blob_fill_single<<<g1, TPB, 0, stream>>>(N, inst, b.fg, b.L1, b.blob_of_root, (int2 *)b.lab_range, b.max_blobs));
     {
-        // patch-sized maps: per-map CTA with the flood state in shared memory; otherwise the generic kernel
-        const size_t budget = 225 * 1024;
-        const size_t state_bytes = (((size_t)N * 2 + 15) & ~(size_t)15), kk_bytes = (((size_t)N * 4 + 15) & ~(size_t)15);
-        const size_t cal_bytes = (((size_t)N * 8 + 15) & ~(size_t)15) + 2 * (WC_NB_BIG * 2 + WC_NB_BIG / 8) +
-                                 (WT_WARPS - 2) * (WC_NB_SMALL * 2 + WC_NB_SMALL / 8);
-        const size_t small_bytes = (size_t)(WT_WARPS - 1) * (WT_SMALL_CAP + 4) * 8;
-        const bool use_kk = state_bytes + kk_bytes + small_bytes + (2048 + 4) * 8 <= budget;
-        const size_t fixed = state_bytes + (use_kk ? kk_bytes : 0) + small_bytes;
-        long long cap = fixed + 64 < budget ? (long long)((budget - fixed) / 8) - 4 : 0;
-        cap = std::min<long long>(cap & ~3ll, 16384);
-        static bool attr = false;
-        if (!attr) {
-            HVN_CUDA(cudaFuncSetAttribute(k_watershed_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget + 64));
-            HVN_CUDA(cudaFuncSetAttribute(k_watershed_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget + 64));
-            HVN_CUDA(cudaFuncSetAttribute(k_watershed_cal, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget + 64));
-            attr = true;
-        }
-        if (cal_bytes <= budget && N < 65535 && b.max_ids < 32000 && g_flood_impl == 0) {
-            L(k_watershed_cal<<<n, WT_WARPS * 32, cal_bytes, stream>>>(H, W, b.dist, b.fg, b.L1, b.size1, b.blob_root, (int4 *)b.bbox,
-                                                                        (const int2 *)b.lab_range, b.max_blobs, inst, st));
-        } else if (cap >= 1024 && N < 65536 && b.max_ids < 32000 && g_flood_impl <= 1) {
-            size_t smem = fixed + (size_t)(cap + 4) * 8;
-            if (use_kk)
-                L(k_watershed_tile<true><<<n, WT_WARPS * 32, smem, stream>>>(H, W, (int)cap, b.dist, b.fg, b.L1, b.size1, b.blob_root,
-                    (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs, (HeapItem *)b.heap, inst, st));
-            else
-                L(k_watershed_tile<false><<<n, WT_WARPS * 32, smem, stream>>>(H, W, (int)cap, b.dist, b.fg, b.L1, b.size1, b.blob_root,
-                    (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs, (HeapItem *)b.heap, inst, st));
-        } else {
-            L(k_watershed<<<dim3((unsigned)b.max_blobs, (unsigned)n), 32, WS_CAP * sizeof(HeapItem), stream>>>(
-                H, W, b.dist, b.fg, b.L1, b.size1, b.blob_root, (int4 *)b.bbox, (const int2 *)b.lab_range, b.max_blobs,
-                (HeapItem *)b.heap, inst, st));
-        }
+        const int fk = postproc_flood(stream, b, n, H, W, inst, FLOOD_AUTO);
+        ++launches;
+        mark(postproc_flood_name(fk));
     }
     // table
     L(k_table_accum<<<g1, TPB, 0, stream>>>(H, W, inst, pred, C, nr_types, (InstAcc *)b.acc, b.tcnt, b.max_ids));
@@ -1222,6 +1277,54 @@ int postproc_run(Arena &arena, cudaStream_t stream, const float *pred, int n, in
         *prof += line;
     }
     return launches;
+}
+
+void postproc_buffers(Arena &arena, int n, int H, int W, int nr_types, PostprocBuffers &b) {
+    const size_t top = arena.top;
+    arena.reset();
+    pp_layout(arena, b, n, H, W, nr_types);
+    arena.top = top;
+}
+
+// flood-only entry: inst = markers where the size-filtered mask is set, 0 elsewhere (what k_marker_labels leaves)
+__global__ void k_mask_markers(int N, const int *__restrict__ markers, const unsigned char *__restrict__ fg_all,
+                               int *__restrict__ inst_all) {
+    int m = blockIdx.y;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < N; p += gridDim.x * blockDim.x) {
+        size_t i = (size_t)m * N + p;
+        inst_all[i] = fg_all[i] ? markers[i] : 0;
+    }
+}
+
+int postproc_flood_only(Arena &arena, cudaStream_t stream, const double *dist, const unsigned char *mask,
+                        const int *markers, int n, int H, int W, int *inst, int choice) {
+    HVN_CHECK(H >= 1 && W >= 1 && n >= 1, -1, "postproc_flood_only: empty input");
+    HVN_CHECK((long long)H * W < (1ll << 30), -1, "postproc_flood_only: map too large (H*W must be < 2^30)");
+    const int N = H * W;
+    const size_t T = (size_t)n * N;
+    PostprocBuffers b;
+    arena.reset();
+    arena.reserve(postproc_workspace_bytes(n, H, W, 0));
+    pp_layout(arena, b, n, H, W, 0);
+    const int TPB = 256;
+    dim3 g1((unsigned)min(cdiv(N, TPB), 1024), (unsigned)n);
+    PPStats *st = (PPStats *)b.stats;
+    k_init_stats<<<cdiv(n, 128), 128, 0, stream>>>(st, n);
+    HVN_CUDA(cudaMemsetAsync(b.size1, 0, T * sizeof(int), stream));
+    k_bbox_init<<<cdiv((size_t)n * b.max_blobs, TPB), TPB, 0, stream>>>((int4 *)b.bbox, (size_t)n * b.max_blobs);
+    k_range_init<<<cdiv((size_t)n * b.max_blobs, TPB), TPB, 0, stream>>>((int2 *)b.lab_range, (size_t)n * b.max_blobs);
+    HVN_CUDA(cudaMemcpyAsync(b.dist, dist, T * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    k_ccl_init<<<g1, TPB, 0, stream>>>(mask, 0, N, b.L1);
+    k_ccl_merge<<<g1, TPB, 0, stream>>>(H, W, b.L1);
+    k_ccl_flatten_count<<<g1, TPB, 0, stream>>>(N, b.L1, b.size1);
+    k_blob_filter<<<g1, TPB, 0, stream>>>(N, b.L1, b.size1, b.fg, b.blob_of_root, b.blob_root, b.max_blobs, st);
+    k_blob_bbox<<<g1, TPB, 0, stream>>>(H, W, b.L1, b.fg, b.blob_of_root, (int4 *)b.bbox, b.max_blobs);
+    k_mask_markers<<<g1, TPB, 0, stream>>>(N, markers, b.fg, inst);
+    k_blob_marker_range<<<g1, TPB, 0, stream>>>(N, inst, b.L1, b.blob_of_root, (int2 *)b.lab_range, b.max_blobs);
+    k_blob_fill_single<<<g1, TPB, 0, stream>>>(N, inst, b.fg, b.L1, b.blob_of_root, (int2 *)b.lab_range, b.max_blobs);
+    const int k = postproc_flood(stream, b, n, H, W, inst, choice);
+    HVN_CUDA(cudaGetLastError());
+    return k;
 }
 
 }  // namespace hvn

@@ -18,10 +18,27 @@ struct PostprocBuffers {
     int *tcnt = nullptr;
 };
 
-void postproc_set_flood_impl(int v);  // test hook: 0 auto, 1 shared-memory heap, 2 global-memory heap
+void postproc_set_flood_impl(int v);  // test hook: 0 auto, 1 no calendar queue, 2 global-memory heap only
 size_t postproc_workspace_bytes(int n, int H, int W, int nr_types);
 // Instance ids a map can hold (ids 1 .. postproc_max_ids - 1): an upper bound on the table rows of one H x W map.
 int postproc_max_ids(int H, int W);
+
+// Watershed flood kernels.  FLOOD_AUTO picks by map size (calendar queue, shared-memory heap with or without the fp32
+// key table, global-memory heap; "flood_impl" narrows the choice); the others force one kernel.
+enum FloodKernel { FLOOD_AUTO = 0, FLOOD_CAL = 1, FLOOD_TILE_KK = 2, FLOOD_TILE = 3, FLOOD_GLOBAL = 4 };
+const char *postproc_flood_name(int k);
+// Launches the flood over the laid-out buffers `b` (markers already in inst, single-label blobs filled).  Returns the
+// FloodKernel launched; a forced kernel that does not fit the map throws Error(-1) without launching.
+int postproc_flood(cudaStream_t stream, const PostprocBuffers &b, int n, int H, int W, int *inst, int choice);
+
+// Test hooks.  postproc_buffers: the stage buffers of the last postproc_run on `arena` for the same (n, H, W, nr_types)
+// (the layout is deterministic; nothing is launched).  postproc_flood_only: the watershed stage alone on caller-owned
+// device maps dist f64 / mask u8 / markers i32 [n,H,W] -> inst i32: the mask's components, the < 10 px filter, boxes,
+// marker ranges, single-label fill and the flood kernel `choice`, the same kernels postproc_run launches.  Marker
+// labels must lie in [0, postproc_max_ids(H, W)).  Returns the FloodKernel launched.
+void postproc_buffers(Arena &arena, int n, int H, int W, int nr_types, PostprocBuffers &b);
+int postproc_flood_only(Arena &arena, cudaStream_t stream, const double *dist, const unsigned char *mask,
+                        const int *markers, int n, int H, int W, int *inst, int choice);
 
 // pred [n,H,W,C] f32 (device) -> inst [n,H,W] i32, table [n,max_rows,10] i64, n_rows [n] i32 (device).
 // Returns the number of kernels launched on `stream`.
