@@ -66,6 +66,14 @@ def precision_code(precision):
     return PRECISIONS[precision]
 
 
+def tta_code(tta):
+    """True -> 1, False -> 0 (libhvn option "tta"); anything but a bool is a ValueError, raised before any device is
+    touched."""
+    if not isinstance(tta, bool):
+        raise ValueError("tta must be True or False, got %r" % (tta,))
+    return int(tta)
+
+
 def _as_ids(a):
     """Instance map as C-contiguous int32; ids that int32 cannot hold are an error, never wrapped."""
     a = np.asarray(a)
@@ -206,10 +214,13 @@ class TilesJob:
 class Context:
     """One libhvn context (one device, one stream).  precision: "highest" (default; fp16 hi + lo operands, three
     products per MAC) or "high" (hi only, one fp16 product per MAC -- TF32-class operand precision); model contexts
-    only, set before any weights are finalised."""
+    only, set before any weights are finalised.  tta (an extension the reference lacks): True runs every patch as its
+    eight dihedral views (4 rotations x optional mirror) and averages their maps, HV vectors mapped back, on the device
+    before post-processing; square patches only; 8x the network work."""
 
-    def __init__(self, device=0, mode=None, nr_types=None, precision="highest"):
+    def __init__(self, device=0, mode=None, nr_types=None, precision="highest", tta=False):
         code = precision_code(precision)
+        tta_on = tta_code(tta)
         self._h = ctypes.c_void_p()
         L = lib()
         if mode is None:
@@ -218,10 +229,13 @@ class Context:
             check(L.hvn_create(int(device), mode.encode(), int(nr_types or 0), ctypes.byref(self._h)))
             if code:
                 self.set_option("precision", code)
+            if tta_on:
+                self.set_option("tta", tta_on)
         self.device = int(device)
         self.mode = mode
         self.nr_types = nr_types
         self.precision = precision
+        self.tta = tta
         for kv in os.environ.get("HVN_OPTS", "").split(","):  # development knobs: HVN_OPTS="key=value,..."
             if "=" in kv and mode is not None:
                 k, v = kv.split("=")

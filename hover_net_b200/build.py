@@ -20,6 +20,7 @@ SOURCES = [
     ("tile.cu", []),
     ("stats.cu", []),
     ("targets.cu", []),
+    ("tta.cu", []),
 ]
 
 

@@ -178,6 +178,15 @@ int hvn_set_option(hvn_ctx *c, const char *key, int64_t value) {
             if (c->model->finalized) c->model->finalize();  // weight planes re-derived (lo dropped / restored); plans rebuilt
         }
     }
+    else if (k == "tta") {
+        HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+        HVN_CHECK(value == 0 || value == 1, HVN_ERR_INVALID, "tta must be 0 (off) or 1 (eight dihedral views, merged)");
+        if (c->model->tta != (int)value) {
+            HVN_CUDA(cudaStreamSynchronize(c->stream));
+            c->model->tta = (int)value;
+            c->model->drop_plans();  // a context keeps the buffers of one mode only
+        }
+    }
     else if (k == "profile") { c->profile = (int)value; if (c->model) c->model->profile_ops = value >= 3 ? 2 : (value >= 2 ? 1 : 0); }
     else throw Error(HVN_ERR_INVALID, "unknown option " + k);
     API_END
@@ -188,6 +197,7 @@ int64_t hvn_get_counter(const hvn_ctx *c, const char *key) {
     std::string k = key;
     if (k == "act_shift") return c->model ? c->model->act_shift : 0;
     if (k == "precision") return c->model ? c->model->precision : 0;
+    if (k == "tta") return c->model ? c->model->tta : 0;
     if (k == "plan_bytes") return c->model ? (int64_t)c->model->last_plan_bytes : 0;
     if (k == "kernel_launches") return (c->model ? c->model->kernel_launches : 0) + c->pp_launches;
     if (k == "tc_launches") return c->model ? c->model->tc_launches : 0;
@@ -986,7 +996,7 @@ int hvn_stage_ms(const hvn_ctx *c, const char *name, float *ms) {
     if (k == "cnn") *ms = c->ms_cnn;
     else if (k == "postproc") *ms = c->ms_pp;
     else if (c->model && c->model->class_ms.count(k)) *ms = (float)c->model->class_ms.at(k);
-    else if (k == "conv_tc" || k == "conv_ref" || k == "conv0" || k == "bnrelu" || k == "head") *ms = 0.f;
+    else if (k == "conv_tc" || k == "conv_ref" || k == "conv0" || k == "bnrelu" || k == "head" || k == "tta") *ms = 0.f;
     else throw Error(HVN_ERR_INVALID, "unknown stage " + k);
     API_END
 }

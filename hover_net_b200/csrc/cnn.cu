@@ -10,6 +10,7 @@
 //   * 2x nearest upsample + skip add is the epilogue of conv_bot / convf;
 //   * TF-"same" padding and valid crops are operand addressing (zero fill outside the view).
 #include "cnn.h"
+#include "tta.h"
 
 #include <algorithm>
 #include <cmath>
@@ -479,13 +480,20 @@ Plan &Model::plan(int B, int H, int W) {
     HVN_CHECK(finalized, -5, "weights not finalised (call hvn_finalize_weights)");
     HVN_CHECK(H == W, -1, "only square patches are supported (reference patch geometry is square)");
     std::string key = std::to_string(B) + "x" + std::to_string(H) + "x" + std::to_string(W) + "p" + std::to_string(conv_path) +
-                      "b" + std::to_string(branch_streams) + "x" + std::to_string(xform) + "f" + std::to_string(fuse_shortcut) + "u" + std::to_string(fuse_up2);
+                      "b" + std::to_string(branch_streams) + "x" + std::to_string(xform) + "f" + std::to_string(fuse_shortcut) + "u" + std::to_string(fuse_up2) + "t" + std::to_string(tta);
     auto it = plans_.find(key);
     if (it != plans_.end()) return *it->second;
     std::unique_ptr<Plan> pl(new Plan());
     Plan &P = *pl;
     P.B = B; P.H = H; P.W = W;
     out_shape(H, W, P.oh, P.ow, P.oc);
+    P.tta = tta;
+    if (tta) {
+        const size_t nv = (size_t)B * H * W * 3, np = (size_t)B * P.oh * P.ow * (nr_types + 3);
+        P.tta_views = dalloc<uint8_t>(nv, P.allocs, false);
+        P.tta_probs = dalloc<float>(np, P.allocs, false);
+        P.bytes += nv + np * sizeof(float);
+    }
 
     auto new_split = [&](int h, int w, int c) {
         SplitRef r;
@@ -672,7 +680,7 @@ Plan &Model::plan(int B, int H, int W) {
     Op head;
     head.kind = Op::HEAD; head.name = "head";
     head.head.nbranch = (int)branches_.size();
-    head.head.B = B; head.head.h = ho; head.head.w_ = ho; head.head.C = P.oc;
+    head.head.B = B; head.head.h = ho; head.head.w_ = ho; head.head.C = tta ? nr_types + 3 : P.oc;
     for (size_t b = 0; b < branches_.size(); ++b) {
         const std::string bp = "decoder." + branches_[b] + ".";
         const int si_ = branch_streams ? (int)b : 0;
@@ -703,29 +711,52 @@ Plan &Model::plan(int B, int H, int W) {
 void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int chunk, cudaStream_t s) {
     HVN_CHECK(finalized, -5, "weights not finalised (call hvn_finalize_weights)");
     HVN_CHECK(B >= 1, -1, "empty batch");
+    HVN_CHECK(!tta || H == W, -1,
+              "test-time augmentation needs square patches (the rotated views of a " + std::to_string(H) + "x" +
+                  std::to_string(W) + " patch are " + std::to_string(W) + "x" + std::to_string(H) + ")");
     int oh, ow, oc;
     out_shape(H, W, oh, ow, oc);
     if (chunk <= 0) chunk = 32;  // sub-batch size: large enough to fill 132 persistent CTAs on the thin decoder layers
+    // inputs per chunk: with TTA a chunk of network patches holds the eight views of chunk / 8 whole inputs
+    const int per = tta ? std::max(1, chunk / 8) : chunk;
     if (!side_[0]) {
         for (auto &st : side_) HVN_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
         HVN_CUDA(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
         for (auto &e : ev_join_) HVN_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
     cudaStream_t main_stream = s;
-    struct Rec { const char *cls; double flops; cudaEvent_t a, b; const Op *op; };
+    struct Rec { const char *cls; double flops; cudaEvent_t a, b; const Op *op; const char *name; };
     std::vector<Rec> recs;
+    // the TTA kernels run on the context stream, outside the op list; profiled as class "tta"
+    auto tta_launch = [&](const char *name, auto &&launch) {
+        Rec r{"tta", 0.0, nullptr, nullptr, nullptr, name};
+        if (profile_ops) {
+            HVN_CUDA(cudaEventCreate(&r.a));
+            HVN_CUDA(cudaEventCreate(&r.b));
+            HVN_CUDA(cudaEventRecord(r.a, main_stream));
+        }
+        launch();
+        ++kernel_launches;
+        if (profile_ops) { HVN_CUDA(cudaEventRecord(r.b, main_stream)); recs.push_back(r); }
+    };
     if (profile_ops) { class_ms.clear(); class_flops.clear(); class_launches.clear(); }
     last_flops = 0;
     last_plan_bytes = 0;
     const Plan *last_plan = nullptr;
     if (conv_path == 2 || profile_ops >= 2) debug_log.clear();
 
-    for (int b0 = 0; b0 < B; b0 += chunk) {
-        int bc = std::min(chunk, B - b0);
+    for (int b0 = 0; b0 < B; b0 += per) {
+        const int nb = std::min(per, B - b0);   // inputs of this chunk
+        const int bc = tta ? 8 * nb : nb;       // network patches of this chunk
         Plan &P = plan(bc, H, W);
         last_flops += P.flops;
         if (&P != last_plan) last_plan_bytes += P.bytes;  // a tail chunk runs a second, smaller plan
         last_plan = &P;
+        const uint8_t *in_c = imgs + (size_t)b0 * H * W * 3;
+        if (tta) {
+            tta_launch("tta_views", [&] { launch_tta_views(in_c, nb, H, P.tta_views, main_stream); });
+            in_c = P.tta_views;
+        }
         int prev_stream = 0;
         bool forked[3] = {true, false, false};
         for (auto &op : P.ops) {
@@ -753,12 +784,10 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
             switch (op.kind) {
             case Op::CONV0:
                 if (stem_tc && conv_path != 1 && conv0_tc_supported(H, W, op.c0_pad, op.c0_out)) {
-                    launch_conv0_tc(imgs + (size_t)b0 * H * W * 3, bc, H, W, op.c0_pad, conv0_tc_w_, op.bn.scale, op.bn.shift,
-                                    op.c0_out, s);
+                    launch_conv0_tc(in_c, bc, H, W, op.c0_pad, conv0_tc_w_, op.bn.scale, op.bn.shift, op.c0_out, s);
                     ++tc_launches;
                 } else
-                    launch_conv0(imgs + (size_t)b0 * H * W * 3, bc, H, W, op.c0_pad, conv0_w_, op.bn.scale, op.bn.shift,
-                                 op.c0_out, s);
+                    launch_conv0(in_c, bc, H, W, op.c0_pad, conv0_w_, op.bn.scale, op.bn.shift, op.c0_out, s);
                 r.cls = "conv0";
                 break;
             case Op::CONV:
@@ -784,8 +813,13 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
                 break;
             case Op::HEAD: {
                 HeadParams hp = op.head;
-                hp.out = out + (size_t)b0 * oh * ow * oc;
-                launch_head(hp, s);
+                if (P.tta) {
+                    hp.out = P.tta_probs;
+                    launch_head_probs(hp, s);
+                } else {
+                    hp.out = out + (size_t)b0 * oh * ow * oc;
+                    launch_head(hp, s);
+                }
                 r.cls = "head";
                 break;
             }
@@ -793,6 +827,10 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
             ++kernel_launches;
             if (profile_ops) { HVN_CUDA(cudaEventRecord(r.b, s)); recs.push_back(r); }
         }
+        if (tta)  // the head ran on the context stream, after the branches joined
+            tta_launch("tta_merge", [&] {
+                launch_tta_merge(P.tta_probs, nb, oh, nr_types, out + (size_t)b0 * oh * ow * oc, main_stream);
+            });
     }
     s = main_stream;
     HVN_CUDA(cudaMemcpyAsync(h_flag_, d_flag_, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
@@ -805,13 +843,13 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
             class_ms[r.cls] += ms; class_flops[r.cls] += r.flops; class_launches[r.cls] += 1;
             if (profile_ops >= 2) {
                 char line[384];
-                const Op &o = *r.op;
-                if (o.kind == Op::CONV)
+                const Op *o = r.op;
+                if (o && o->kind == Op::CONV)
                     snprintf(line, sizeof(line), "%-44s %-8s k%dx%d s%d cin%-4d cout%-4d out%dx%d box=%dx%d bn=%d %8.4f ms %8.2f GFLOP %7.1f TFLOP/s\n",
-                             o.name.c_str(), r.cls, o.cp.w.kh, o.cp.w.kw, o.cp.stride, o.cp.w.cin, o.cp.w.cout, o.cp.ho, o.cp.wo,
-                             o.tc.bw, o.tc.bh, o.tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f));
+                             o->name.c_str(), r.cls, o->cp.w.kh, o->cp.w.kw, o->cp.stride, o->cp.w.cin, o->cp.w.cout, o->cp.ho, o->cp.wo,
+                             o->tc.bw, o->tc.bh, o->tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f));
                 else
-                    snprintf(line, sizeof(line), "%-44s %-8s %8.4f ms\n", o.name.c_str(), r.cls, ms);
+                    snprintf(line, sizeof(line), "%-44s %-8s %8.4f ms\n", o ? o->name.c_str() : r.name, r.cls, ms);
                 debug_log += line;
             }
             cudaEventDestroy(r.a); cudaEventDestroy(r.b);

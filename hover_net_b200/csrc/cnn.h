@@ -45,6 +45,11 @@ struct Op {
 
 struct Plan {
     int B = 0, H = 0, W = 0, oh = 0, ow = 0, oc = 0;
+    // tta: B network patches are the eight views of B / 8 inputs; the stem reads tta_views, the head stores
+    // probabilities (k_head_probs) into tta_probs [B,oh,ow,nr_types+3], which k_tta_merge reduces into the output
+    int tta = 0;
+    uint8_t *tta_views = nullptr;
+    float *tta_probs = nullptr;
     std::vector<Op> ops;
     std::vector<void *> allocs;
     size_t bytes = 0;
@@ -79,9 +84,14 @@ class Model {
     // product per MAC -- the operand precision of TF32.  Accumulation, residual sums, BN and heads stay fp32 in both.
     // Weights are re-finalised on a change.
     int precision = 0;
+    // Test-time augmentation.  1: every input patch runs as its eight dihedral views (tta.h), whose maps are brought
+    // back to the input's frame and averaged on the device; each chunk holds the views of chunk / 8 inputs (at least
+    // one).  0 (default): the plain forward.  Square patches only.
+    int tta = 0;
     // true if the last forward() stored a value outside the fp16 range (valid after the stream was synchronised)
     bool range_overflow() const { return h_flag_ && *h_flag_ != 0; }
     void reset_range_flag(cudaStream_t s);  // after the host has seen (and reported) an overflow
+    void drop_plans() { plans_.clear(); }   // frees the cached plans' buffers (the caller has synchronised)
 
     void load(const std::string &name, const float *data, int ndim, const int64_t *shape);
     void finalize();

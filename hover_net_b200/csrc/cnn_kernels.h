@@ -30,6 +30,8 @@ void launch_conv0_tc(const uint8_t *img, int B, int H, int W, int pad, const Con
 void launch_bnrelu(const RawRef &in, int B, const float *scale, const float *shift, const SplitRef &out,
                    cudaStream_t s);
 void launch_head(const HeadParams &P, cudaStream_t s);
+// the heads with the TP branch's out_ch softmax probabilities in place of its argmax: C = out_ch(tp) + 3
+void launch_head_probs(const HeadParams &P, cudaStream_t s);
 void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRef &out, cudaStream_t s);
 
 // wgmma path (conv_tc.cu).  tc_plan() decides eligibility and builds the TMA descriptors once per

@@ -7,6 +7,7 @@
 //   k_bnrelu     BatchNorm(eval)+ReLU raw fp32 -> split (dense-unit preact / blk_bna, net_utils.py:98-99,135-142)
 //   k_head       1x1 64->out_ch + bias for every branch, softmax / argmax, concat to [B,h,w,C]
 //                (reference net_desc.py:62-68, run_desc.py:185-194)
+//   k_head_probs the same with the TP softmax probabilities stored instead of their argmax (test-time augmentation)
 #include "common.cuh"
 #include "conv_epilogue.cuh"
 #include "cnn_kernels.h"
@@ -309,8 +310,10 @@ void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRe
 }
 
 // ------------------------------------------------------------------------------------------------
-// heads.  feat[b] is the BN+ReLU'd 64-channel map of branch b (order tp?, np, hv).
-__global__ void __launch_bounds__(128) k_head(HeadParams P) {
+// heads.  feat[b] is the BN+ReLU'd 64-channel map of branch b (order tp?, np, hv).  PROBS: the TP branch stores its
+// out_ch softmax probabilities instead of their argmax (test-time augmentation merges those); NP and HV come from the
+// same code in both variants.
+template <bool PROBS> __device__ __forceinline__ void head_body(const HeadParams &P) {
     __shared__ float s_w[3][HVN_MAX_TYPES][64];
     __shared__ float s_b[3][HVN_MAX_TYPES];
     for (int i = threadIdx.x; i < 3 * HVN_MAX_TYPES * 64; i += blockDim.x) {
@@ -358,6 +361,8 @@ __global__ void __launch_bounds__(128) k_head(HeadParams P) {
             for (int o = 0; o < och; ++o) { e[o] = expf(logit[o] - mx); sum += e[o]; }
             if (P.kind[b] == HEAD_NP) {
                 out[oc++] = e[1] / sum;  // softmax(np)[..., 1]
+            } else if (PROBS) {          // softmax(tp)
+                for (int o = 0; o < och; ++o) out[oc++] = e[o] / sum;
             } else {                     // argmax(softmax(tp)), first maximal index, as float
                 int best = 0;
                 float bv = e[0] / sum;
@@ -367,10 +372,16 @@ __global__ void __launch_bounds__(128) k_head(HeadParams P) {
         }
     }
 }
+__global__ void __launch_bounds__(128) k_head(HeadParams P) { head_body<false>(P); }
+__global__ void __launch_bounds__(128) k_head_probs(HeadParams P) { head_body<true>(P); }
 
 void launch_head(const HeadParams &P, cudaStream_t s) {
     long long M = (long long)P.B * P.h * P.w_;
     k_head<<<cdiv(M, 128), 128, 0, s>>>(P);
+}
+void launch_head_probs(const HeadParams &P, cudaStream_t s) {
+    long long M = (long long)P.B * P.h * P.w_;
+    k_head_probs<<<cdiv(M, 128), 128, 0, s>>>(P);
 }
 
 }  // namespace hvn

@@ -19,13 +19,17 @@ def convert_pytorch_checkpoint(net_state_dict):
 
 class HoVerNet(object):
     """precision: "highest" (default) or "high" -- see `_lib.Context`.  An extension: the reference has no such
-    argument (its PyTorch convolutions run in TF32 on this GPU by default)."""
+    argument (its PyTorch convolutions run in TF32 on this GPU by default).
+    tta: False (default) or True -- test-time augmentation over the eight dihedral views, see `_lib.Context`.  An
+    extension too: the reference has no test-time augmentation."""
 
-    def __init__(self, input_ch=3, nr_types=None, freeze=False, mode="original", device=None, precision="highest"):
+    def __init__(self, input_ch=3, nr_types=None, freeze=False, mode="original", device=None, precision="highest",
+                 tta=False):
         assert mode == "original" or mode == "fast", \
             "Unknown mode `%s` for HoVerNet %s. Only support `original` or `fast`." % (mode, "")
         assert input_ch == 3, "only RGB input is supported"
         _lib.precision_code(precision)  # ValueError before a context exists
+        _lib.tta_code(tta)
         self.mode = mode
         self.freeze = freeze
         self.nr_types = nr_types
@@ -35,7 +39,8 @@ class HoVerNet(object):
             import os
             device = int(os.environ.get("LOCAL_RANK", "0"))
         self.precision = precision
-        self.ctx = _lib.Context(device, mode, nr_types, precision=precision)
+        self.tta = tta
+        self.ctx = _lib.Context(device, mode, nr_types, precision=precision, tta=tta)
         self._loaded = False
 
     # ---- torch.nn.Module look-alikes used by reference infer/base.py:64-70
@@ -75,7 +80,7 @@ class HoVerNet(object):
         raise RuntimeError("call models.hovernet.run_desc.infer_step(batch, model) -- the fused device path")
 
 
-def create_model(mode=None, *, precision="highest", **kwargs):
+def create_model(mode=None, *, precision="highest", tta=False, **kwargs):
     if mode not in ["original", "fast"]:
         assert "Unknown Model Mode %s" % mode
-    return HoVerNet(mode=mode, precision=precision, **kwargs)
+    return HoVerNet(mode=mode, precision=precision, tta=tta, **kwargs)

@@ -15,6 +15,11 @@ precision.  `highest` forms fp32-grade products (fp16 hi + lo operands); `high` 
 that feeds a convolution as one fp16 value and forms one product per multiply-accumulate, with fp32 accumulation --
 the operand precision the reference itself gets from PyTorch's default TF32 convolutions on this GPU -- for a third of
 the tensor-core work.  A non-default value is passed to `create_model` through `method_args["method"]["model_args"]`.
+
+Extension the reference CLI lacks: `--tta` (test-time augmentation) runs every patch as its eight dihedral views
+(4 rotations x optional mirror) and averages their maps on the device, the HV vectors mapped back to the patch's
+frame, before post-processing: eight times the network work.  When given, `"tta": True` is added to `model_args`;
+tile and WSI modes take it from the model.
 """
 import argparse
 import logging
@@ -36,6 +41,7 @@ def _top_parser():
     ap.add_argument("--nr_post_proc_workers", default="16")
     ap.add_argument("--batch_size", default="32")
     ap.add_argument("--precision", default="highest", choices=["highest", "high"])
+    ap.add_argument("--tta", action="store_true")
     return ap
 
 
@@ -88,6 +94,8 @@ def parse(argv, nr_gpus=1):
     }
     if args.precision != "highest":  # the default leaves model_args exactly as the reference builds them
         method_args["method"]["model_args"]["precision"] = args.precision
+    if args.tta:
+        method_args["method"]["model_args"]["tta"] = True
     run_args = {
         "batch_size": int(args.batch_size) * max(1, nr_gpus),
         "nr_inference_workers": int(args.nr_inference_workers),

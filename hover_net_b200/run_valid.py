@@ -8,7 +8,10 @@ counts are summed on the host.  Prints np_acc, np_dice, tp_dice_<k> (with --nr_t
 names.  hv_mse sums in float64 where the reference sums in float32.
 
 usage: python -m hover_net_b200.run_valid --model_path CKPT --valid_dir DIR [--valid_dir DIR ...]
-       [--model_mode original|fast] [--nr_types N] [--batch_size B] [--precision highest|high] [--json OUT]
+       [--model_mode original|fast] [--nr_types N] [--batch_size B] [--precision highest|high] [--tta] [--json OUT]
+
+--tta scores the checkpoint with test-time augmentation (the eight dihedral views of every patch, merged on the
+device), so that its effect on these scalars can be measured on the user's own labelled patches.
 """
 import argparse
 import ctypes
@@ -30,6 +33,7 @@ def parse_args(argv=None):
     ap.add_argument("--valid_dir", action="append", required=True, help="directory of .npy patches (repeatable)")
     ap.add_argument("--batch_size", type=int, default=16)
     ap.add_argument("--precision", default="highest", choices=["highest", "high"])
+    ap.add_argument("--tta", action="store_true", help="test-time augmentation: eight dihedral views, merged")
     ap.add_argument("--json", default=None, help="also write the scalars to this JSON file")
     return ap.parse_args(argv)
 
@@ -51,7 +55,7 @@ def run(args):
         raise SystemExit("no .npy patches found in %s" % args.valid_dir)
     nr_types = args.nr_types or None
     input_shape, mask_shape = SHAPES[args.model_mode]
-    net = net_desc.create_model(mode=args.model_mode, nr_types=nr_types, precision=args.precision)
+    net = net_desc.create_model(mode=args.model_mode, nr_types=nr_types, precision=args.precision, tta=args.tta)
     # checkpoint formats as in infer/base.py: an .npz of arrays or the reference's torch file with a "desc" entry
     if str(args.model_path).endswith(".npz"):
         state = dict(np.load(args.model_path))

@@ -83,6 +83,15 @@ int hvn_finalize_weights(hvn_ctx *ctx);
  *                      (HVN_ERR_RANGE, "act_shift") are the same.  A change synchronises the context, re-derives the
  *                      weights and drops the cached plans; setting 0 again reproduces "highest" bit for bit.
  *                      Any other value is HVN_ERR_INVALID;
+ *                      "tta" = 0 (default) | 1: test-time augmentation.  Every input patch runs as its 8 dihedral
+ *                      views V_t(x) = rot90(t >= 4 ? flip(x, 1) : x, t % 4) (numpy, axes (0, 1)); each view's map is
+ *                      brought back (rot90(., -(t % 4)), then flip(., 1) if t >= 4; HV vector (h, v) <- (-v, h)
+ *                      t % 4 times, then h <- -h if t >= 4), and per output value the 8 are summed in view order in
+ *                      fp32 and scaled by 1/8; TP is the argmax (first maximal index) of the mean softmax
+ *                      probabilities.  Output layout, post-processing and the range rules are unchanged; a chunk
+ *                      holds the views of max(1, chunk / 8) inputs.  Square patches only (H != W is
+ *                      HVN_ERR_INVALID).  A change synchronises the context and drops the cached plans; 0 again is
+ *                      the plain forward bit for bit.  Any other value is HVN_ERR_INVALID;
  *                      "profile" = 0 | 1 | 2 (see hvn_stage_ms);
  *                      tuning knobs: "tc_seg_chunks" (64-channel slices per accumulation segment), "tc_block_n",
  *                      "tc_prefetch" (L2 prefetch distance in K-slices for flat operands, 0 = off), "tc_xf_trunc"
@@ -95,9 +104,10 @@ const char *hvn_debug_log(const hvn_ctx *ctx);
 /* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing and contour kernels), "tile_table_rows" (rows
  * of padded instance tables the last hvn_infer_tiles* group of two or more images held in the context's workspace:
  * min(rows_cap, H*W/6 + 8) per image, 84 B each), "last_flops" (algorithmic 2*MACs of the
- * last forward), "precision" (0 | 1), "plan_bytes" (device bytes of the activation buffers of the plan(s) the last
+ * last forward; with "tta" = 1 the 8 views' work), "precision" (0 | 1), "tta" (0 | 1), "plan_bytes" (device bytes of
+ * the activation buffers, and with "tta" = 1 the per-chunk view and probability workspace, of the plan(s) the last
  * forward ran); with option "profile" = 2 also "launches:<class>" and "flops:<class>" for
- * class in {conv_tc, conv_ref, conv0, bnrelu, head} (see hvn_stage_ms). */
+ * class in {conv_tc, conv_ref, conv0, bnrelu, head, tta} (see hvn_stage_ms). */
 int64_t hvn_get_counter(const hvn_ctx *ctx, const char *key);
 
 /* ---- geometry of reference HoVerNet.forward (net_desc.py:101-145) for an in_h x in_w patch. */
@@ -251,7 +261,7 @@ int hvn_timer_stop(hvn_ctx *ctx, float *ms);
 /* device time (ms) of the last forward / postproc call.  option "profile" = 1: name in
  * {"cnn","postproc"} (whole stage, CUDA events on the context stream).  "profile" = 2 additionally
  * brackets every CNN launch with its own event pair and sums per kernel class:
- * {"conv_tc","conv_ref","conv0","bnrelu","head"}. */
+ * {"conv_tc","conv_ref","conv0","bnrelu","head","tta"} ("tta": the view and merge kernels of option "tta"). */
 int hvn_stage_ms(const hvn_ctx *ctx, const char *name, float *ms);
 
 #ifdef __cplusplus
