@@ -463,6 +463,42 @@ class Context:
         check(L.hvn_valid_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
                               _ptr(d_counts), _ptr(d_sse), _ptr(d_flags)))
 
+    _VALID_LOSS_ARGS = _VALID_ARGS + [ctypes.c_void_p, ctypes.c_void_p]
+
+    def valid_loss(self, imgs_u8, inst, type_map=None, want_probs=False):
+        """`valid` plus the reference's training-loss sums on the same eval-mode forward (hvn_valid_loss).  Returns
+        (counts, hv_sse, flags) as `valid` does, then sums float64 [10 + (1 + 3*nr_types if typed)] (layout in
+        include/hvn.h; run_desc.loss_scalars turns them into the loss values) and, with want_probs, the probability
+        map float32 [B,h,w,4+nr_types] = [np p0, np p1, hv x, hv y, tp p0..] (else None).  A type id outside
+        0..nr_types-1 inside the output crop raises HvnError (HVN_ERR_INVALID)."""
+        x = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
+        B, H, W, C = x.shape
+        assert C == 3
+        a = _as_ids(inst)
+        t = None if type_map is None or not self.nr_types else _as_ids(type_map)
+        if a.shape != (B, H, W) or (t is not None and t.shape != (B, H, W)):
+            raise ValueError("inst / type maps must be [B,H,W] = %s" % ((B, H, W),))
+        nt = int(self.nr_types or 0)
+        counts = np.zeros((3 + 2 * nt,), dtype=np.int64)
+        sse = np.zeros((1,), dtype=np.float64)
+        flags = np.zeros((B,), dtype=np.int32)
+        sums = np.zeros((10 + (1 + 3 * nt if nt else 0),), dtype=np.float64)
+        probs = None
+        if want_probs:
+            oh, ow, _ = self.out_shape(H, W)
+            probs = np.empty((B, oh, ow, 4 + nt), dtype=np.float32)
+        L = lib()
+        L.hvn_valid_loss.argtypes = self._VALID_LOSS_ARGS
+        check(self._retry_range(lambda: L.hvn_valid_loss(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
+                                                         _ptr(sse), _ptr(flags), _ptr(sums), _ptr(probs))))
+        return counts, float(sse[0]), flags, sums, probs
+
+    def valid_loss_dev(self, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags, d_sums, d_probs=None):
+        L = lib()
+        L.hvn_valid_loss_dev.argtypes = self._VALID_LOSS_ARGS
+        check(L.hvn_valid_loss_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
+                                   _ptr(d_counts), _ptr(d_sse), _ptr(d_flags), _ptr(d_sums), _ptr(d_probs)))
+
     def mem_get_info(self):
         """(free, total) device bytes of this context's device (hvn_mem_info)."""
         free, total = ctypes.c_size_t(), ctypes.c_size_t()

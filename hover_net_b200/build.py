@@ -21,6 +21,7 @@ SOURCES = [
     ("stats.cu", []),
     ("targets.cu", []),
     ("tta.cu", []),
+    ("loss.cu", []),
 ]
 
 

@@ -7,6 +7,7 @@
 
 #include "../../include/hvn.h"
 #include "cnn.h"
+#include "loss.h"
 #include "postproc.h"
 #include "stats.h"
 #include "targets.h"
@@ -26,6 +27,7 @@ struct hvn_ctx {
     Arena stats_arena;             // pair-table workspace of hvn_inst_pairs*
     Arena targets_arena;           // workspace of hvn_targets* and hvn_valid*
     Arena valid_arena;             // maps and counts of hvn_valid*
+    Arena loss_arena;              // per-block partials of hvn_valid_loss*
     Arena group_arena;             // slot table, padded instance tables and slot-order maps of the tile-group path
     void *pin = nullptr;           // pinned staging of the tile-group slot table (uploaded stream-ordered)
     size_t pin_bytes = 0;
@@ -35,7 +37,7 @@ struct hvn_ctx {
     int profile = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t tev[2] = {nullptr, nullptr};
-    float ms_cnn = 0.f, ms_pp = 0.f;
+    float ms_cnn = 0.f, ms_pp = 0.f, ms_loss = 0.f;
     long long pp_launches = 0;
     std::string pp_log;  // per-kernel post-processing times of the last call ("profile" >= 3)
     std::string log_out;
@@ -105,6 +107,7 @@ void hvn_destroy(hvn_ctx *c) {
     c->stats_arena.release();
     c->targets_arena.release();
     c->valid_arena.release();
+    c->loss_arena.release();
     c->group_arena.release();
     if (c->pin) cudaFreeHost(c->pin);
     if (c->pin_ev) cudaEventDestroy(c->pin_ev);
@@ -230,10 +233,10 @@ int hvn_out_shape(const hvn_ctx *c, int in_h, int in_w, int *out_h, int *out_w, 
 }
 
 // ---------------------------------------------------------------------------------------------------
-static void run_forward(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, float *out) {
+static void run_forward(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, float *out, int layout = OUT_PLAIN) {
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
-    c->model->forward(imgs, B, H, W, out, c->chunk, c->stream);
+    c->model->forward(imgs, B, H, W, out, c->chunk, c->stream, layout);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[1], c->stream));
 }
 static void run_postproc(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
@@ -906,6 +909,92 @@ int hvn_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_
     API_END
 }
 
+// Forward with every probability, targets, loss sums and counts of one batch, enqueued on the context stream; the
+// caller synchronises and checks.  probs (may be null) receives the [B,h,w,4+nt] map by a copy of kind pk.
+static void run_valid_loss(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H,
+                           int W, int64_t *counts, double *sse, double *sums, float *probs, cudaMemcpyKind pk,
+                           int32_t *flags, TargetWork &w, LossWork &lw) {
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    const int nt = c->model->nr_types;
+    HVN_CHECK(imgs && inst && counts && sse && sums && flags, HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(nt == 0 || type, HVN_ERR_INVALID, "a model with nr_types > 0 needs a type map");
+    int oh, ow, oc;
+    c->model->out_shape(H, W, oh, ow, oc);
+    check_targets_args(B, H, W, oh, ow);
+    oc = nt + 4;
+    const size_t opx = (size_t)B * oh * ow, px = (size_t)B * H * W;
+    c->valid_arena.reset();
+    c->valid_arena.reserve(opx * oc * 4 + px * 8 + 1024);
+    float *d_probs = c->valid_arena.take<float>(opx * oc);
+    float *d_hv = c->valid_arena.take<float>(px * 2);
+    HVN_CUDA(cudaMemsetAsync(counts, 0, (size_t)(3 + 2 * nt) * 8, c->stream));
+    run_forward(c, imgs, B, H, W, d_probs, OUT_FULL);
+    targets_run(c->targets_arena, c->stream, inst, B, H, W, oh, ow, d_hv, flags, w);
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[2], c->stream));
+    loss_reduce(c->loss_arena, c->stream, d_probs, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, nt, sums,
+                (long long *)counts, lw);
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[3], c->stream));
+    HVN_CUDA(cudaMemcpyAsync(sse, sums + LS_HV_SQ, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+    if (probs) HVN_CUDA(cudaMemcpyAsync(probs, d_probs, opx * oc * 4, pk, c->stream));
+}
+// After the context stream has been synchronised.
+static void finish_valid_loss(hvn_ctx *c, const TargetWork &w, const LossWork &lw) {
+    finish_profile(c, true, false);
+    if (c->profile) HVN_CUDA(cudaEventElapsedTime(&c->ms_loss, c->ev[2], c->ev[3]));
+    check_range(c);
+    check_targets_result(w);
+    int err = 0;
+    HVN_CUDA(cudaMemcpy(&err, lw.err, sizeof(int), cudaMemcpyDeviceToHost));
+    HVN_CHECK(!err, HVN_ERR_INVALID,
+              "type id outside 0.." + std::to_string(c->model->nr_types - 1) + " inside the output crop");
+}
+
+int hvn_valid_loss_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                       int64_t *counts, double *sse, int32_t *flags, double *sums, float *probs) {
+    API_BEGIN
+    use(c);
+    TargetWork w;
+    LossWork lw;
+    run_valid_loss(c, imgs, inst, type, B, H, W, counts, sse, sums, probs, cudaMemcpyDeviceToDevice, flags, w, lw);
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    finish_valid_loss(c, w, lw);
+    API_END
+}
+
+int hvn_valid_loss(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                   int64_t *counts, double *sse, int32_t *flags, double *sums, float *probs) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    HVN_CHECK(imgs && inst && counts && sse && flags && sums, HVN_ERR_INVALID, "null buffer");
+    check_targets_args(B, H, W, 1, 1);
+    const int nt = c->model->nr_types;
+    const size_t px = (size_t)B * H * W, nc = 3 + 2 * (size_t)nt, ns = loss_nsums(nt);
+    c->io_arena.reset();
+    c->io_arena.reserve(px * 3 + px * 4 * (nt ? 2 : 1) + (nc + 1 + ns) * 8 + (size_t)B * 4 + 8 + 4096);
+    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
+    int32_t *d_inst = c->io_arena.take<int32_t>(px);
+    int32_t *d_type = nt && type ? c->io_arena.take<int32_t>(px) : nullptr;
+    int64_t *d_counts = c->io_arena.take<int64_t>(nc);
+    double *d_sse = c->io_arena.take<double>(1);
+    double *d_sums = c->io_arena.take<double>(ns);
+    int32_t *d_flags = c->io_arena.take<int32_t>(B);
+    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
+    if (d_type) HVN_CUDA(cudaMemcpyAsync(d_type, type, px * 4, cudaMemcpyHostToDevice, c->stream));
+    TargetWork w;
+    LossWork lw;
+    run_valid_loss(c, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_sums, probs, cudaMemcpyDeviceToHost, d_flags,
+                   w, lw);
+    HVN_CUDA(cudaMemcpyAsync(counts, d_counts, nc * 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(sse, d_sse, 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(sums, d_sums, ns * 8, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    finish_valid_loss(c, w, lw);
+    API_END
+}
+
 // ---------------------------------------------------------------------------------------------------
 int hvn_malloc(hvn_ctx *c, size_t bytes, void **p) {
     API_BEGIN
@@ -995,6 +1084,7 @@ int hvn_stage_ms(const hvn_ctx *c, const char *name, float *ms) {
     std::string k = name;
     if (k == "cnn") *ms = c->ms_cnn;
     else if (k == "postproc") *ms = c->ms_pp;
+    else if (k == "loss") *ms = c->ms_loss;
     else if (c->model && c->model->class_ms.count(k)) *ms = (float)c->model->class_ms.at(k);
     else if (k == "conv_tc" || k == "conv_ref" || k == "conv0" || k == "bnrelu" || k == "head" || k == "tta") *ms = 0.f;
     else throw Error(HVN_ERR_INVALID, "unknown stage " + k);

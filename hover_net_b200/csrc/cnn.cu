@@ -708,14 +708,17 @@ Plan &Model::plan(int B, int H, int W) {
     return *plans_[key];
 }
 
-void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int chunk, cudaStream_t s) {
+void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int chunk, cudaStream_t s, int layout) {
     HVN_CHECK(finalized, -5, "weights not finalised (call hvn_finalize_weights)");
     HVN_CHECK(B >= 1, -1, "empty batch");
     HVN_CHECK(!tta || H == W, -1,
               "test-time augmentation needs square patches (the rotated views of a " + std::to_string(H) + "x" +
                   std::to_string(W) + " patch are " + std::to_string(W) + "x" + std::to_string(H) + ")");
+    HVN_CHECK(layout == OUT_PLAIN || layout == OUT_FULL, -1, "bad forward output layout");
+    const bool full = layout == OUT_FULL;
     int oh, ow, oc;
     out_shape(H, W, oh, ow, oc);
+    if (full) oc = nr_types + 4;
     if (chunk <= 0) chunk = 32;  // sub-batch size: large enough to fill 132 persistent CTAs on the thin decoder layers
     // inputs per chunk: with TTA a chunk of network patches holds the eight views of chunk / 8 whole inputs
     const int per = tta ? std::max(1, chunk / 8) : chunk;
@@ -749,6 +752,11 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
         const int nb = std::min(per, B - b0);   // inputs of this chunk
         const int bc = tta ? 8 * nb : nb;       // network patches of this chunk
         Plan &P = plan(bc, H, W);
+        if (tta && full && !P.tta_full) {
+            const size_t n = (size_t)bc * oh * ow * oc;
+            P.tta_full = dalloc<float>(n, P.allocs, false);
+            P.bytes += n * sizeof(float);
+        }
         last_flops += P.flops;
         if (&P != last_plan) last_plan_bytes += P.bytes;  // a tail chunk runs a second, smaller plan
         last_plan = &P;
@@ -813,7 +821,11 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
                 break;
             case Op::HEAD: {
                 HeadParams hp = op.head;
-                if (P.tta) {
+                if (full) {
+                    hp.C = oc;
+                    hp.out = P.tta ? P.tta_full : out + (size_t)b0 * oh * ow * oc;
+                    launch_head_full(hp, s);
+                } else if (P.tta) {
                     hp.out = P.tta_probs;
                     launch_head_probs(hp, s);
                 } else {
@@ -829,7 +841,9 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
         }
         if (tta)  // the head ran on the context stream, after the branches joined
             tta_launch("tta_merge", [&] {
-                launch_tta_merge(P.tta_probs, nb, oh, nr_types, out + (size_t)b0 * oh * ow * oc, main_stream);
+                float *o = out + (size_t)b0 * oh * ow * oc;
+                if (full) launch_tta_merge_full(P.tta_full, nb, oh, nr_types, o, main_stream);
+                else launch_tta_merge(P.tta_probs, nb, oh, nr_types, o, main_stream);
             });
     }
     s = main_stream;

@@ -50,6 +50,8 @@ struct Plan {
     int tta = 0;
     uint8_t *tta_views = nullptr;
     float *tta_probs = nullptr;
+    // the views' k_head_full maps [B,oh,ow,nr_types+4] for a forward with layout OUT_FULL, allocated by the first one
+    float *tta_full = nullptr;
     std::vector<Op> ops;
     std::vector<void *> allocs;
     size_t bytes = 0;
@@ -98,8 +100,11 @@ class Model {
     void out_shape(int H, int W, int &oh, int &ow, int &oc) const;
     // builds (and caches) the plan for a sub-batch geometry
     Plan &plan(int B, int H, int W);
-    // runs B patches: imgs u8 [B,H,W,3] (device) -> out f32 [B,oh,ow,oc] (device)
-    void forward(const uint8_t *imgs, int B, int H, int W, float *out, int chunk, cudaStream_t s);
+    // runs B patches: imgs u8 [B,H,W,3] (device) -> out f32 [B,oh,ow,oc] (device).  layout OUT_FULL (the validation
+    // loss) stores every probability instead, out f32 [B,oh,ow,nr_types+4] = [np p0, np p1, hv x, hv y, tp p0..];
+    // np p1 and hv equal the OUT_PLAIN forward's bit for bit, with and without tta.
+    void forward(const uint8_t *imgs, int B, int H, int W, float *out, int chunk, cudaStream_t s,
+                 int layout = OUT_PLAIN);
 
     long long kernel_launches = 0, tc_launches = 0;
     // per-kernel-class device time of the last forward() when profile_ops != 0 (CUDA events per launch)

@@ -8,6 +8,8 @@
 namespace hvn {
 
 enum HeadKind { HEAD_TP = 0, HEAD_NP = 1, HEAD_HV = 2 };
+// what the heads store per pixel: launch_head, launch_head_probs, launch_head_full
+enum HeadOut { OUT_PLAIN = 0, OUT_PROBS = 1, OUT_FULL = 2 };
 
 struct HeadParams {
     int nbranch = 0;
@@ -32,6 +34,9 @@ void launch_bnrelu(const RawRef &in, int B, const float *scale, const float *shi
 void launch_head(const HeadParams &P, cudaStream_t s);
 // the heads with the TP branch's out_ch softmax probabilities in place of its argmax: C = out_ch(tp) + 3
 void launch_head_probs(const HeadParams &P, cudaStream_t s);
+// every softmax probability, in a fixed order whatever the branch order: C = 4 + out_ch(tp) =
+// [np p0, np p1, hv x, hv y, tp p0 .. p(nt-1)] (the layout of the validation loss)
+void launch_head_full(const HeadParams &P, cudaStream_t s);
 void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRef &out, cudaStream_t s);
 
 // wgmma path (conv_tc.cu).  tc_plan() decides eligibility and builds the TMA descriptors once per

@@ -8,6 +8,7 @@
 //   k_head       1x1 64->out_ch + bias for every branch, softmax / argmax, concat to [B,h,w,C]
 //                (reference net_desc.py:62-68, run_desc.py:185-194)
 //   k_head_probs the same with the TP softmax probabilities stored instead of their argmax (test-time augmentation)
+//   k_head_full  every softmax probability, [np p0, np p1, hv x, hv y, tp p0..] (validation loss)
 #include "common.cuh"
 #include "conv_epilogue.cuh"
 #include "cnn_kernels.h"
@@ -310,10 +311,12 @@ void launch_up2_add(const RawRef &in, int B, const SplitRef &skip, const SplitRe
 }
 
 // ------------------------------------------------------------------------------------------------
-// heads.  feat[b] is the BN+ReLU'd 64-channel map of branch b (order tp?, np, hv).  PROBS: the TP branch stores its
-// out_ch softmax probabilities instead of their argmax (test-time augmentation merges those); NP and HV come from the
-// same code in both variants.
-template <bool PROBS> __device__ __forceinline__ void head_body(const HeadParams &P) {
+// heads.  feat[b] is the BN+ReLU'd 64-channel map of branch b (order tp?, np, hv).  OUT_PLAIN: [tp argmax?, np p1,
+// hv x, hv y].  OUT_PROBS: the TP branch stores its out_ch softmax probabilities instead of their argmax (test-time
+// augmentation merges those).  OUT_FULL: [np p0, np p1, hv x, hv y, tp p0..] (the validation loss needs every
+// probability).  NP, HV and the TP probabilities come from the same code in all three variants.
+template <int OUT> __device__ __forceinline__ void head_body(const HeadParams &P) {
+    constexpr bool PROBS = OUT != OUT_PLAIN;
     __shared__ float s_w[3][HVN_MAX_TYPES][64];
     __shared__ float s_b[3][HVN_MAX_TYPES];
     for (int i = threadIdx.x; i < 3 * HVN_MAX_TYPES * 64; i += blockDim.x) {
@@ -334,6 +337,7 @@ template <bool PROBS> __device__ __forceinline__ void head_body(const HeadParams
     float *out = P.out + m * P.C;
     int oc = 0;
     for (int b = 0; b < P.nbranch; ++b) {
+        if (OUT == OUT_FULL) oc = P.kind[b] == HEAD_NP ? 0 : (P.kind[b] == HEAD_HV ? 2 : 4);
         const SplitRef &f = P.feat[b];
         long long fo = n * f.sN + (long long)y * f.sH + (long long)x * f.sW;
         float logit[HVN_MAX_TYPES];
@@ -360,6 +364,7 @@ template <bool PROBS> __device__ __forceinline__ void head_body(const HeadParams
             float sum = 0.f, e[HVN_MAX_TYPES];
             for (int o = 0; o < och; ++o) { e[o] = expf(logit[o] - mx); sum += e[o]; }
             if (P.kind[b] == HEAD_NP) {
+                if (OUT == OUT_FULL) out[oc++] = e[0] / sum;
                 out[oc++] = e[1] / sum;  // softmax(np)[..., 1]
             } else if (PROBS) {          // softmax(tp)
                 for (int o = 0; o < och; ++o) out[oc++] = e[o] / sum;
@@ -372,8 +377,9 @@ template <bool PROBS> __device__ __forceinline__ void head_body(const HeadParams
         }
     }
 }
-__global__ void __launch_bounds__(128) k_head(HeadParams P) { head_body<false>(P); }
-__global__ void __launch_bounds__(128) k_head_probs(HeadParams P) { head_body<true>(P); }
+__global__ void __launch_bounds__(128) k_head(HeadParams P) { head_body<OUT_PLAIN>(P); }
+__global__ void __launch_bounds__(128) k_head_probs(HeadParams P) { head_body<OUT_PROBS>(P); }
+__global__ void __launch_bounds__(128) k_head_full(HeadParams P) { head_body<OUT_FULL>(P); }
 
 void launch_head(const HeadParams &P, cudaStream_t s) {
     long long M = (long long)P.B * P.h * P.w_;
@@ -382,6 +388,10 @@ void launch_head(const HeadParams &P, cudaStream_t s) {
 void launch_head_probs(const HeadParams &P, cudaStream_t s) {
     long long M = (long long)P.B * P.h * P.w_;
     k_head_probs<<<cdiv(M, 128), 128, 0, s>>>(P);
+}
+void launch_head_full(const HeadParams &P, cudaStream_t s) {
+    long long M = (long long)P.B * P.h * P.w_;
+    k_head_full<<<cdiv(M, 128), 128, 0, s>>>(P);
 }
 
 }  // namespace hvn

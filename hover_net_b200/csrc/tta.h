@@ -17,5 +17,9 @@ void launch_tta_views(const uint8_t *imgs, int n, int S, uint8_t *views, cudaStr
 // brought-back views are summed in view order in fp32 and scaled by 1/8; TP takes the argmax of the summed
 // probabilities (first maximal index).
 void launch_tta_merge(const float *probs, int n, int h, int nr_types, float *out, cudaStream_t s);
+// probs f32 [8n,h,h,nr_types+4] in k_head_full's layout (np p0, np p1, h, v, tp p0..) -> out f32 [n,h,h,nr_types+4],
+// same layout: every channel is the same view-order fp32 sum scaled by 1/8, so np p1, h and v equal
+// launch_tta_merge's bit for bit.
+void launch_tta_merge_full(const float *probs, int n, int h, int nr_types, float *out, cudaStream_t s);
 
 }  // namespace hvn

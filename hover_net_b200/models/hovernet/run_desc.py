@@ -1,5 +1,6 @@
 """Drop-in for reference `models/hovernet/run_desc.py`: `infer_step` (:171-197), `valid_step` (:113-167) and
-`proc_valid_step_output` (:263-344, scalars only)."""
+`proc_valid_step_output` (:263-344, scalars only), plus `loss_scalars`: the loss values `train_step` (:12-109)
+tracks, from the sums of hvn_valid_loss."""
 import numpy as np
 
 
@@ -95,3 +96,38 @@ def proc_valid_step_output(raw_data, nr_types=None):
     nr_pixels = n * np.size(true_np[0])
     scalar = valid_scalars(correct, inter, total, type_counts, sse, nr_pixels)
     return {"scalar": scalar, "image": {}}
+
+
+# opt.py extra_info["loss"]: every term has weight 1
+LOSS_OPTS = {"np": {"bce": 1, "dice": 1}, "hv": {"mse": 1, "msge": 1}, "tp": {"bce": 1, "dice": 1}}
+
+
+def loss_scalars(sums, nr_pixels, loss_opts=None):
+    """The reference's training loss (train_step with utils.py xentropy_loss, dice_loss, mse_loss, msge_loss) from
+    the sums of `Context.valid_loss` (layout in include/hvn.h; 10 entries untyped, 11 + 3*nr_types typed) over
+    nr_pixels = B*h*w output pixels.  Sums added over several batches give the loss of the set as one batch.
+    Returns {"loss_<branch>_<term>": value, ..., "overall_loss": weighted sum} in train_step's order: branches tp
+    (when typed), np, hv; terms in loss_opts' order (default: opt.py's weights, all 1).  Float64 throughout."""
+    s = np.asarray(sums, np.float64)
+    n = float(nr_pixels)
+    nt = (len(s) - 11) // 3 if len(s) > 10 else 0
+
+    def dice(i, l, r):
+        return float(np.sum(1.0 - (2.0 * i + 1e-3) / (l + r + 1e-3)))
+
+    terms = {
+        "np": {"bce": s[0] / n, "dice": dice(s[1:3], s[3:5], s[5:7])},
+        "hv": {"mse": s[7] / (2.0 * n), "msge": s[8] / (2.0 * s[9] + 1.0e-8)},
+    }
+    if nt:
+        terms["tp"] = {"bce": s[10] / n,
+                       "dice": dice(s[11:11 + nt], s[11 + nt:11 + 2 * nt], s[11 + 2 * nt:11 + 3 * nt])}
+    opts = LOSS_OPTS if loss_opts is None else loss_opts
+    out, total = {}, 0.0
+    for branch in (("tp",) if nt else ()) + ("np", "hv"):
+        for name, weight in opts[branch].items():
+            v = float(terms[branch][name])
+            out["loss_%s_%s" % (branch, name)] = v
+            total += weight * v
+    out["overall_loss"] = total
+    return out

@@ -8,10 +8,18 @@ counts are summed on the host.  Prints np_acc, np_dice, tp_dice_<k> (with --nr_t
 names.  hv_mse sums in float64 where the reference sums in float32.
 
 usage: python -m hover_net_b200.run_valid --model_path CKPT --valid_dir DIR [--valid_dir DIR ...]
-       [--model_mode original|fast] [--nr_types N] [--batch_size B] [--precision highest|high] [--tta] [--json OUT]
+       [--model_mode original|fast] [--nr_types N] [--batch_size B] [--precision highest|high] [--tta] [--loss]
+       [--json OUT]
 
 --tta scores the checkpoint with test-time augmentation (the eight dihedral views of every patch, merged on the
 device), so that its effect on these scalars can be measured on the user's own labelled patches.
+
+--loss also prints the reference's training loss on these patches (train_step's loss_<branch>_<term> names and
+overall_loss, opt.py's weights), after the scalars above: each batch runs hvn_valid_loss instead of hvn_valid, the
+per-batch sums are added in float64, and the loss formulas are applied once to the set's sums, so the values are those
+of the whole set as one batch, whatever --batch_size is.  The network runs in eval mode (running BatchNorm
+statistics), so this is the validation loss: train_step evaluates the same formulas with batch statistics.  hv_mse
+then comes from the loss pass's sum, equal to hvn_valid's to float64 reordering.
 """
 import argparse
 import ctypes
@@ -34,6 +42,7 @@ def parse_args(argv=None):
     ap.add_argument("--batch_size", type=int, default=16)
     ap.add_argument("--precision", default="highest", choices=["highest", "high"])
     ap.add_argument("--tta", action="store_true", help="test-time augmentation: eight dihedral views, merged")
+    ap.add_argument("--loss", action="store_true", help="also the training loss (loss_*, overall_loss) on these patches")
     ap.add_argument("--json", default=None, help="also write the scalars to this JSON file")
     return ap.parse_args(argv)
 
@@ -80,6 +89,7 @@ def run(args):
         img, inst, typ = img.reshape(B, H, W, 3), inst.reshape(B, H, W), typ.reshape(B, H, W)
         counts = np.zeros((3 + 2 * (nr_types or 0),), np.int64)
         sse = 0.0
+        sums = 0.0
         for lo in range(0, len(files), B):
             n = min(B, len(files) - lo)
             for i in range(n):
@@ -87,7 +97,11 @@ def run(args):
                 img[i], inst[i] = a, b
                 if t is not None:
                     typ[i] = t
-            c, s, flags = ctx.valid(img[:n], inst[:n], typ[:n] if nr_types else None)
+            if args.loss:
+                c, s, flags, ls, _ = ctx.valid_loss(img[:n], inst[:n], typ[:n] if nr_types else None)
+                sums = sums + ls
+            else:
+                c, s, flags = ctx.valid(img[:n], inst[:n], typ[:n] if nr_types else None)
             targets.raise_for_flags(flags, names=files[lo:lo + n])
             counts += c
             sse += s
@@ -95,7 +109,11 @@ def run(args):
         for p in (p_img, p_inst, p_type):
             ctx.free_host(p)
     tc = [(counts[3 + 2 * k], counts[4 + 2 * k]) for k in range(nr_types)] if nr_types else None
-    return run_desc.valid_scalars(counts[0], counts[1], counts[2], tc, sse, len(files) * mask_shape[0] * mask_shape[1])
+    nr_pixels = len(files) * mask_shape[0] * mask_shape[1]
+    scalars = run_desc.valid_scalars(counts[0], counts[1], counts[2], tc, sse, nr_pixels)
+    if args.loss:
+        scalars.update(run_desc.loss_scalars(sums, nr_pixels))
+    return scalars
 
 
 def main(argv=None):

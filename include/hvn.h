@@ -244,6 +244,30 @@ int hvn_valid(hvn_ctx *ctx, const uint8_t *imgs_host, const int32_t *inst_host, 
 int hvn_valid_dev(hvn_ctx *ctx, const uint8_t *imgs_dev, const int32_t *inst_dev, const int32_t *type_dev, int B,
                   int H, int W, int64_t *counts_dev, double *hv_sse_dev, int32_t *flags_dev);
 
+/* ---- validation loss: the reference's training objective (run_desc.py train_step; models/hovernet/utils.py
+ * xentropy_loss, dice_loss, mse_loss, msge_loss) evaluated on the engine's eval-mode forward, on the same batch and
+ * arguments as hvn_valid.  counts, hv_sse and flags are hvn_valid's (counts exactly; hv_sse to fp64 reordering).
+ * sums double [10 + (nr_types ? 1 + 3*nr_types : 0)], over the B x h x w output crop, fp32 per-pixel terms added in
+ * fp64 (p the softmax, t the one-hot target, q = p / sum_c p clamped to [1e-7, 1 - 1e-7] in fp32):
+ *   0 np_ce = sum -log q_true;  1, 2 I_c = sum p_c t_c;  3, 4 L_c = sum p_c;  5, 6 R_c = sum t_c  (NP, t = inst > 0)
+ *   7 hv_sq = sum (pred_hv - true_hv)^2 over both channels
+ *   8 msge_num = sum f ((G_h(p) - G_h(t))^2 + (G_v(p) - G_v(t))^2), G_h / G_v the 5x5 kernels of get_sobel_kernel(5)
+ *     on HV channels 0 / 1 as a cross-correlation, zero padding at the crop border;  9 focus = sum f, f = inst > 0
+ *   with nr_types > 0: 10 tp_ce, then I_k (11 + k), L_k (11 + nt + k), R_k (11 + 2 nt + k) against type.
+ * The reduction is deterministic (per-block partials in fixed slots, one fixed-order pass; no floating-point atomics):
+ * equal inputs give bit-identical sums whatever "chunk" is.  probs (may be NULL) receives float32 [B,h,w,4+nr_types]
+ * = [np p0, np p1, hv x, hv y, tp p0..] (with "tta" = 1 the view mean of every channel); np p1 and hv equal the plain
+ * forward's bit for bit.  HVN_ERR_INVALID on a type id outside 0..nr_types-1 inside the crop (the reference's
+ * F.one_hot raises; hvn_valid ignores such ids).  Device workspace (context-owned, grow-only): (4 + nr_types) * 4 B
+ * per output pixel for the probabilities, 8 B per input pixel for the HV targets, 8 * sums B per 32 x 32 tile of the
+ * crop for the partials, and hvn_targets' 60 B per input pixel.  Both variants synchronise the context stream. */
+int hvn_valid_loss(hvn_ctx *ctx, const uint8_t *imgs_host, const int32_t *inst_host, const int32_t *type_host, int B,
+                   int H, int W, int64_t *counts_host, double *hv_sse_host, int32_t *flags_host, double *sums_host,
+                   float *probs_host);
+int hvn_valid_loss_dev(hvn_ctx *ctx, const uint8_t *imgs_dev, const int32_t *inst_dev, const int32_t *type_dev, int B,
+                       int H, int W, int64_t *counts_dev, double *hv_sse_dev, int32_t *flags_dev, double *sums_dev,
+                       float *probs_dev);
+
 /* ---- device memory / stream helpers for callers without a CUDA binding of their own. */
 int hvn_malloc(hvn_ctx *ctx, size_t bytes, void **dev_ptr);
 int hvn_free(hvn_ctx *ctx, void *dev_ptr);
@@ -259,7 +283,8 @@ int hvn_mem_info(hvn_ctx *ctx, size_t *free_bytes, size_t *total_bytes);
 int hvn_timer_start(hvn_ctx *ctx);
 int hvn_timer_stop(hvn_ctx *ctx, float *ms);
 /* device time (ms) of the last forward / postproc call.  option "profile" = 1: name in
- * {"cnn","postproc"} (whole stage, CUDA events on the context stream).  "profile" = 2 additionally
+ * {"cnn","postproc","loss"} (whole stage, CUDA events on the context stream; "loss": the reduction of the last
+ * hvn_valid_loss* call).  "profile" = 2 additionally
  * brackets every CNN launch with its own event pair and sums per kernel class:
  * {"conv_tc","conv_ref","conv0","bnrelu","head","tta"} ("tta": the view and merge kernels of option "tta"). */
 int hvn_stage_ms(const hvn_ctx *ctx, const char *name, float *ms);
