@@ -19,6 +19,62 @@ class HvnError(RuntimeError):
         self.code = code
 
 
+# The C ABI of include/hvn.h as ctypes sees it: name -> (restype, argtypes).  Every pointer is c_void_p, `const char *`
+# is c_char_p; lib() applies the table when the library loads.
+_P, _S, _I, _I64, _SZ = ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t
+_VALID = [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P]
+_TILES_ARGS = [_P, _I, _P, _P, _I, _I, _P, _P, _P, _I64, _P, _P, _I64, _P]
+PROTOTYPES = {
+    "hvn_abi_version": (_I, []),
+    "hvn_last_error": (_S, []),
+    "hvn_create": (_I, [_I, _S, _I, _P]),
+    "hvn_destroy": (None, [_P]),
+    "hvn_num_params": (_I, [_P]),
+    "hvn_param_info": (_I, [_P, _I, _P, _P, _P]),
+    "hvn_load_param": (_I, [_P, _S, _P, _I, _P]),
+    "hvn_finalize_weights": (_I, [_P]),
+    "hvn_set_option": (_I, [_P, _S, _I64]),
+    "hvn_debug_log": (_S, [_P]),
+    "hvn_get_counter": (_I64, [_P, _S]),
+    "hvn_out_shape": (_I, [_P, _I, _I, _P, _P, _P]),
+    "hvn_forward": (_I, [_P, _P, _I, _I, _I, _P]),
+    "hvn_forward_dev": (_I, [_P, _P, _I, _I, _I, _P]),
+    "hvn_create_postproc": (_I, [_I, _P]),
+    "hvn_postproc": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P]),
+    "hvn_postproc_dev": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P]),
+    "hvn_contours_dev": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _I64, _P]),
+    "hvn_postproc_contours": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I64, _P]),
+    "hvn_forward_postproc": (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _I, _P]),
+    "hvn_forward_postproc_dev": (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _I, _P]),
+    "hvn_tile_grid": (_I, [_P, _I, _I, _I, _P, _P]),
+    "hvn_tile_predict_dev": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "hvn_infer_tile": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _I, _P, _P, _I64, _P]),
+    "hvn_infer_tiles": (_I, _TILES_ARGS),
+    "hvn_infer_tiles_dev": (_I, _TILES_ARGS),
+    "hvn_pack_tables_dev": (_I, [_P, _P, _P, _I, _I, _P, _I64, _P]),
+    "hvn_get_stream": (_I, [_P, _P]),
+    "hvn_inst_pairs": (_I, [_P, _P, _P, _I, _I, _I, _P, _I64, _P]),
+    "hvn_inst_pairs_dev": (_I, [_P, _P, _P, _I, _I, _I, _P, _I64, _P]),
+    "hvn_targets": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "hvn_targets_dev": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "hvn_valid": (_I, _VALID),
+    "hvn_valid_dev": (_I, _VALID),
+    "hvn_valid_loss": (_I, _VALID + [_P, _P]),
+    "hvn_valid_loss_dev": (_I, _VALID + [_P, _P]),
+    "hvn_malloc": (_I, [_P, _SZ, _P]),
+    "hvn_free": (_I, [_P, _P]),
+    "hvn_malloc_host": (_I, [_P, _SZ, _P]),
+    "hvn_free_host": (_I, [_P, _P]),
+    "hvn_memcpy_h2d": (_I, [_P, _P, _P, _SZ]),
+    "hvn_memcpy_d2h": (_I, [_P, _P, _P, _SZ]),
+    "hvn_sync": (_I, [_P]),
+    "hvn_mem_info": (_I, [_P, _P, _P]),
+    "hvn_timer_start": (_I, [_P]),
+    "hvn_timer_stop": (_I, [_P, _P]),
+    "hvn_stage_ms": (_I, [_P, _S, _P]),
+}
+
+
 def lib():
     global _lib
     if _lib is None:
@@ -26,18 +82,9 @@ def lib():
             raise HvnError(-2, "libhvn.so is not built (run `python -c 'import __graft_entry__ as g; g.build()'`); "
                                "this package has no CPU fallback")
         L = ctypes.CDLL(LIB_PATH)
-        L.hvn_last_error.restype = ctypes.c_char_p
-        L.hvn_debug_log.restype = ctypes.c_char_p
-        L.hvn_debug_log.argtypes = [ctypes.c_void_p]
-        L.hvn_get_counter.restype = ctypes.c_int64
-        L.hvn_get_counter.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
-        L.hvn_set_option.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int64]
-        for name in ("hvn_malloc", "hvn_malloc_host"):
-            getattr(L, name).argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p)]
-        for name in ("hvn_memcpy_h2d", "hvn_memcpy_d2h"):
-            getattr(L, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t]
-        for name in ("hvn_free", "hvn_free_host"):
-            getattr(L, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        for name, (restype, argtypes) in PROTOTYPES.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -45,6 +92,17 @@ def lib():
 def check(rc):
     if rc != 0:
         raise HvnError(rc, lib().hvn_last_error().decode("utf-8", "replace"))
+
+
+def _retry_capacity(what, attempt):
+    """Runs attempt() -> (rc, result) until rc is not HVN_ERR_CAPACITY (-4), at most 4 times, and returns result; any
+    other failure raises.  On -4, attempt has taken the exact sizes the call reported for its next run."""
+    for _attempt in range(4):
+        rc, result = attempt()
+        if rc != -4:
+            check(rc)
+            return result
+    raise HvnError(-4, "%s: capacity retries exhausted" % what)
 
 
 def _ptr(a):
@@ -123,11 +181,6 @@ def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None
     return out
 
 
-_TILES_ARGS = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
-               ctypes.c_void_p]
-
-
 class TilesJob:
     """A tile group enqueued with hvn_infer_tiles_dev (Context.infer_tiles_begin).  result() synchronises and returns
     what Context.infer_tiles returns.  A capacity failure reruns the group through Context.infer_tiles with the sizes the
@@ -147,12 +200,10 @@ class TilesJob:
         self.d = {k: (ctx.malloc(b) if b else None) for k, b in sizes.items()}
         try:
             ctx.h2d(self.d["img"], self.packed, self.packed.nbytes)
-            L = lib()
-            L.hvn_infer_tiles_dev.argtypes = _TILES_ARGS
-            check(L.hvn_infer_tiles_dev(ctx._h, n, _ptr(self.d["img"]), _ptr(self.shapes), int(patch_in), int(batch),
-                                        _ptr(self.d["pred"]), _ptr(self.d["inst"]), _ptr(self.d["table"]),
-                                        int(self.rows_cap), _ptr(self.d["ro"]), _ptr(self.d["pts"]),
-                                        int(self.pts_cap if contours else 0), _ptr(self.d["po"])))
+            check(lib().hvn_infer_tiles_dev(ctx._h, n, _ptr(self.d["img"]), _ptr(self.shapes), int(patch_in), int(batch),
+                                            _ptr(self.d["pred"]), _ptr(self.d["inst"]), _ptr(self.d["table"]),
+                                            int(self.rows_cap), _ptr(self.d["ro"]), _ptr(self.d["pts"]),
+                                            int(self.pts_cap if contours else 0), _ptr(self.d["po"])))
         except Exception:
             self._free()
             raise
@@ -316,17 +367,18 @@ class Context:
         n, H, W, C = p.shape
         if max_rows is None:
             max_rows = max(16, H * W // 64)
-        while True:
+
+        def attempt():
+            nonlocal max_rows
             inst = np.empty((n, H, W), dtype=np.int32)
             table = np.zeros((n, max_rows, ROW_LEN), dtype=np.int64)
             nrows = np.zeros((n,), dtype=np.int32)
             rc = lib().hvn_postproc(self._h, _ptr(p), n, H, W, C, int(nr_types or 0), _ptr(inst), _ptr(table),
                                     int(max_rows), _ptr(nrows))
-            if rc == -4:  # HVN_ERR_CAPACITY: retry with the exact size
+            if rc == -4:
                 max_rows = int(nrows.max())
-                continue
-            check(rc)
-            return inst, table, nrows
+            return rc, (inst, table, nrows)
+        return _retry_capacity("postproc", attempt)
 
     def postproc_contours(self, pred, nr_types=None, max_rows=None, pts_cap=None):
         """postproc + device contour tracing: (inst, table, nrows, offs [n*max_rows+1], pts [total,2])."""
@@ -338,37 +390,27 @@ class Context:
             max_rows = max(16, H * W // 64)
         if pts_cap is None:
             pts_cap = max(4096, n * H * W // 16)
-        for _attempt in range(4):  # at most: grow the table once, then the point buffer once
+
+        def attempt():  # a capacity failure grows the table once, then the point buffer once
+            nonlocal max_rows, pts_cap
             inst = np.empty((n, H, W), dtype=np.int32)
             table = np.zeros((n, max_rows, ROW_LEN), dtype=np.int64)
             nrows = np.zeros((n,), dtype=np.int32)
             offs = np.zeros((n * max_rows + 1,), dtype=np.int32)
             pts = np.empty((pts_cap, 2), dtype=np.int32)
-            L = lib()
-            L.hvn_postproc_contours.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
-                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
-            rc = L.hvn_postproc_contours(self._h, _ptr(p), n, H, W, C, int(nr_types or 0), _ptr(inst), _ptr(table),
-                                         int(max_rows), _ptr(nrows), _ptr(pts), int(pts_cap), _ptr(offs))
-            if rc == -4:  # HVN_ERR_CAPACITY: the table or the point buffer was too small -- retry with exact sizes
+            rc = lib().hvn_postproc_contours(self._h, _ptr(p), n, H, W, C, int(nr_types or 0), _ptr(inst), _ptr(table),
+                                             int(max_rows), _ptr(nrows), _ptr(pts), int(pts_cap), _ptr(offs))
+            if rc == -4:
                 if int(nrows.max()) > max_rows:
                     max_rows = int(nrows.max())
                 else:
                     pts_cap = int(offs[-1])
-                continue
-            check(rc)
-            return inst, table, nrows, offs, pts[: int(offs[-1])]
-        raise HvnError(-4, "postproc_contours: capacity retries exhausted")
+            return rc, (inst, table, nrows, offs, pts[: int(offs[-1])])
+        return _retry_capacity("postproc_contours", attempt)
 
     def contours_dev(self, d_inst, d_table, d_nrows, n, H, W, max_rows, d_pts, pts_cap, d_offs):
-        L = lib()
-        L.hvn_contours_dev.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
-                                       ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
-        check(L.hvn_contours_dev(self._h, _ptr(d_inst), _ptr(d_table), _ptr(d_nrows), n, H, W, int(max_rows), _ptr(d_pts),
-                                 int(pts_cap), _ptr(d_offs)))
-
-    _PAIRS_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                   ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+        check(lib().hvn_contours_dev(self._h, _ptr(d_inst), _ptr(d_table), _ptr(d_nrows), n, H, W, int(max_rows),
+                                     _ptr(d_pts), int(pts_cap), _ptr(d_offs)))
 
     def inst_pairs(self, true, pred=None, cap=None):
         """Contingency table of instance maps true/pred [H,W] or [n,H,W] (ids >= 0, 0 = background; pred None = all
@@ -384,35 +426,28 @@ class Context:
         n, H, W = t.shape
         if cap is None:
             cap = max(1024, n * H * W // 64)
-        L = lib()
-        L.hvn_inst_pairs.argtypes = self._PAIRS_ARGS
-        for _attempt in range(2):
+
+        def attempt():
+            nonlocal cap
             rows = np.empty((cap, 3), dtype=np.int64)
             offs = np.zeros((n + 1,), dtype=np.int64)
-            rc = L.hvn_inst_pairs(self._h, _ptr(t), _ptr(p), n, H, W, _ptr(rows), int(cap), _ptr(offs))
-            if rc == -4:  # HVN_ERR_CAPACITY: retry with the exact size
+            rc = lib().hvn_inst_pairs(self._h, _ptr(t), _ptr(p), n, H, W, _ptr(rows), int(cap), _ptr(offs))
+            if rc == -4:
                 cap = int(offs[-1])
-                continue
-            check(rc)
-            rows = rows[: int(offs[-1])]
-            m = np.repeat(np.arange(n), np.diff(offs))
-            return rows[np.lexsort((rows[:, 1], rows[:, 0], m))], offs
-        raise HvnError(-4, "inst_pairs: capacity retries exhausted")
+            return rc, (rows[: int(offs[-1])], offs)
+        rows, offs = _retry_capacity("inst_pairs", attempt)
+        m = np.repeat(np.arange(n), np.diff(offs))
+        return rows[np.lexsort((rows[:, 1], rows[:, 0], m))], offs
 
     def inst_pairs_dev(self, d_true, d_pred, n, H, W, d_pairs, cap, d_offs):
         """Device-pointer variant (d_pred may be None).  Returns False on HVN_ERR_CAPACITY (offs is valid on the
         device then: retry with cap >= offs[n]), True on success; raises on any other error."""
-        L = lib()
-        L.hvn_inst_pairs_dev.argtypes = self._PAIRS_ARGS
-        rc = L.hvn_inst_pairs_dev(self._h, _ptr(d_true), _ptr(d_pred), int(n), int(H), int(W), _ptr(d_pairs),
-                                  int(cap), _ptr(d_offs))
+        rc = lib().hvn_inst_pairs_dev(self._h, _ptr(d_true), _ptr(d_pred), int(n), int(H), int(W), _ptr(d_pairs),
+                                      int(cap), _ptr(d_offs))
         if rc == -4:
             return False
         check(rc)
         return True
-
-    _TARGETS_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
 
     def targets(self, inst, crop_shape):
         """Full-size HV targets of instance maps inst [H,W] or [n,H,W] (the reference's gen_instance_hv_map):
@@ -423,24 +458,18 @@ class Context:
         n, H, W = a.shape
         hv = np.empty((n, H, W, 2), dtype=np.float32)
         flags = np.zeros((n,), dtype=np.int32)
-        L = lib()
-        L.hvn_targets.argtypes = self._TARGETS_ARGS
-        check(L.hvn_targets(self._h, _ptr(a), n, H, W, int(crop_shape[0]), int(crop_shape[1]), _ptr(hv), _ptr(flags)))
+        check(lib().hvn_targets(self._h, _ptr(a), n, H, W, int(crop_shape[0]), int(crop_shape[1]), _ptr(hv), _ptr(flags)))
         return hv, flags
 
     def targets_dev(self, d_inst, n, H, W, crop_h, crop_w, d_hv, d_flags):
-        L = lib()
-        L.hvn_targets_dev.argtypes = self._TARGETS_ARGS
-        check(L.hvn_targets_dev(self._h, _ptr(d_inst), int(n), int(H), int(W), int(crop_h), int(crop_w), _ptr(d_hv),
-                                _ptr(d_flags)))
+        check(lib().hvn_targets_dev(self._h, _ptr(d_inst), int(n), int(H), int(W), int(crop_h), int(crop_w), _ptr(d_hv),
+                                    _ptr(d_flags)))
 
-    _VALID_ARGS = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                   ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    # argument list of hvn_valid_loss*, for callers that set a function's argtypes themselves (as _TILES_ARGS)
+    _VALID_LOSS_ARGS = PROTOTYPES["hvn_valid_loss"][1]
 
-    def valid(self, imgs_u8, inst, type_map=None):
-        """One validation batch through forward, targets and counts on the device (model contexts).  imgs uint8
-        [B,H,W,3], inst / type_map int32 [B,H,W] at the network input size.  Returns (counts int64 [3 + 2*nr_types]
-        = correct, inter, total, then inter_k, total_k per type; hv_sse float; flags int32 [B])."""
+    def _valid_args(self, imgs_u8, inst, type_map):
+        """The inputs of a validation batch as the C ABI takes them, and its zeroed counts, hv_sse and flags."""
         x = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
         B, H, W, C = x.shape
         assert C == 3
@@ -449,21 +478,21 @@ class Context:
         if a.shape != (B, H, W) or (t is not None and t.shape != (B, H, W)):
             raise ValueError("inst / type maps must be [B,H,W] = %s" % ((B, H, W),))
         counts = np.zeros((3 + 2 * int(self.nr_types or 0),), dtype=np.int64)
-        sse = np.zeros((1,), dtype=np.float64)
-        flags = np.zeros((B,), dtype=np.int32)
-        L = lib()
-        L.hvn_valid.argtypes = self._VALID_ARGS
-        check(self._retry_range(lambda: L.hvn_valid(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
-                                                    _ptr(sse), _ptr(flags))))
+        return x, a, t, counts, np.zeros((1,), dtype=np.float64), np.zeros((B,), dtype=np.int32)
+
+    def valid(self, imgs_u8, inst, type_map=None):
+        """One validation batch through forward, targets and counts on the device (model contexts).  imgs uint8
+        [B,H,W,3], inst / type_map int32 [B,H,W] at the network input size.  Returns (counts int64 [3 + 2*nr_types]
+        = correct, inter, total, then inter_k, total_k per type; hv_sse float; flags int32 [B])."""
+        x, a, t, counts, sse, flags = self._valid_args(imgs_u8, inst, type_map)
+        B, H, W, _ = x.shape
+        check(self._retry_range(lambda: lib().hvn_valid(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
+                                                        _ptr(sse), _ptr(flags))))
         return counts, float(sse[0]), flags
 
     def valid_dev(self, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags):
-        L = lib()
-        L.hvn_valid_dev.argtypes = self._VALID_ARGS
-        check(L.hvn_valid_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
-                              _ptr(d_counts), _ptr(d_sse), _ptr(d_flags)))
-
-    _VALID_LOSS_ARGS = _VALID_ARGS + [ctypes.c_void_p, ctypes.c_void_p]
+        check(lib().hvn_valid_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
+                                  _ptr(d_counts), _ptr(d_sse), _ptr(d_flags)))
 
     def valid_loss(self, imgs_u8, inst, type_map=None, want_probs=False):
         """`valid` plus the reference's training-loss sums on the same eval-mode forward (hvn_valid_loss).  Returns
@@ -471,40 +500,26 @@ class Context:
         include/hvn.h; run_desc.loss_scalars turns them into the loss values) and, with want_probs, the probability
         map float32 [B,h,w,4+nr_types] = [np p0, np p1, hv x, hv y, tp p0..] (else None).  A type id outside
         0..nr_types-1 inside the output crop raises HvnError (HVN_ERR_INVALID)."""
-        x = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
-        B, H, W, C = x.shape
-        assert C == 3
-        a = _as_ids(inst)
-        t = None if type_map is None or not self.nr_types else _as_ids(type_map)
-        if a.shape != (B, H, W) or (t is not None and t.shape != (B, H, W)):
-            raise ValueError("inst / type maps must be [B,H,W] = %s" % ((B, H, W),))
+        x, a, t, counts, sse, flags = self._valid_args(imgs_u8, inst, type_map)
+        B, H, W, _ = x.shape
         nt = int(self.nr_types or 0)
-        counts = np.zeros((3 + 2 * nt,), dtype=np.int64)
-        sse = np.zeros((1,), dtype=np.float64)
-        flags = np.zeros((B,), dtype=np.int32)
         sums = np.zeros((10 + (1 + 3 * nt if nt else 0),), dtype=np.float64)
         probs = None
         if want_probs:
             oh, ow, _ = self.out_shape(H, W)
             probs = np.empty((B, oh, ow, 4 + nt), dtype=np.float32)
-        L = lib()
-        L.hvn_valid_loss.argtypes = self._VALID_LOSS_ARGS
-        check(self._retry_range(lambda: L.hvn_valid_loss(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
-                                                         _ptr(sse), _ptr(flags), _ptr(sums), _ptr(probs))))
+        check(self._retry_range(lambda: lib().hvn_valid_loss(self._h, _ptr(x), _ptr(a), _ptr(t), B, H, W, _ptr(counts),
+                                                             _ptr(sse), _ptr(flags), _ptr(sums), _ptr(probs))))
         return counts, float(sse[0]), flags, sums, probs
 
     def valid_loss_dev(self, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags, d_sums, d_probs=None):
-        L = lib()
-        L.hvn_valid_loss_dev.argtypes = self._VALID_LOSS_ARGS
-        check(L.hvn_valid_loss_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
-                                   _ptr(d_counts), _ptr(d_sse), _ptr(d_flags), _ptr(d_sums), _ptr(d_probs)))
+        check(lib().hvn_valid_loss_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
+                                       _ptr(d_counts), _ptr(d_sse), _ptr(d_flags), _ptr(d_sums), _ptr(d_probs)))
 
     def mem_get_info(self):
         """(free, total) device bytes of this context's device (hvn_mem_info)."""
         free, total = ctypes.c_size_t(), ctypes.c_size_t()
-        L = lib()
-        L.hvn_mem_info.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)]
-        check(L.hvn_mem_info(self._h, ctypes.byref(free), ctypes.byref(total)))
+        check(lib().hvn_mem_info(self._h, ctypes.byref(free), ctypes.byref(total)))
         return int(free.value), int(total.value)
 
     def tile_grid(self, H, W, patch_in):
@@ -523,18 +538,16 @@ class Context:
             max_rows = max(16, H * W // 64)
         if pts_cap is None:
             pts_cap = max(4096, H * W // 16)
-        L = lib()
-        L.hvn_infer_tile.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                     ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
-                                     ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
-        for _attempt in range(4):
+
+        def attempt():
+            nonlocal max_rows, pts_cap
             pred = np.empty((H, W, oc), dtype=np.float32) if want_pred else None
             inst = np.empty((H, W), dtype=np.int32)
             table = np.zeros((max_rows, ROW_LEN), dtype=np.int64)
             nrows = np.zeros((1,), dtype=np.int32)
             offs = np.zeros((max_rows + 1,), dtype=np.int32) if contours else None
             pts = np.empty((pts_cap, 2), dtype=np.int32) if contours else None
-            rc = self._retry_range(lambda: L.hvn_infer_tile(
+            rc = self._retry_range(lambda: lib().hvn_infer_tile(
                 self._h, _ptr(x), H, W, int(patch_in), int(batch), _ptr(pred), _ptr(inst), _ptr(table), int(max_rows),
                 _ptr(nrows), _ptr(pts), int(pts_cap if contours else 0), _ptr(offs)))
             if rc == -4:
@@ -542,11 +555,9 @@ class Context:
                     max_rows = int(nrows[0])
                 else:
                     pts_cap = int(offs[-1])
-                continue
-            check(rc)
             n = int(nrows[0])
-            return pred, inst, table[:n], offs, (pts[: int(offs[-1])] if contours else None)
-        raise HvnError(-4, "infer_tile: capacity retries exhausted")
+            return rc, (pred, inst, table[:n], offs, (pts[: int(offs[-1])] if contours else None))
+        return _retry_capacity("infer_tile", attempt)
 
     def infer_tiles(self, imgs, patch_in, batch=0, want_pred=True, contours=True, rows_cap=None, pts_cap=None):
         """A group of RGB images [H_i,W_i,3] of any sizes through the device tile path in one stream of batches
@@ -561,31 +572,30 @@ class Context:
         r0, p0 = tiles_sizes(shapes)
         rows_cap = r0 if rows_cap is None else int(rows_cap)
         pts_cap = p0 if pts_cap is None else int(pts_cap)
-        L = lib()
-        L.hvn_infer_tiles.argtypes = _TILES_ARGS
-        for _attempt in range(4):  # at most: grow the table once, then the point buffer once
+
+        def attempt():  # a capacity failure grows the table once, then the point buffer once
+            nonlocal rows_cap, pts_cap
             pred = np.empty((px * oc,), dtype=np.float32) if want_pred else None
             inst = np.empty((px,), dtype=np.int32)
             table = np.empty((rows_cap, ROW_LEN), dtype=np.int64)
             ro = np.zeros((n + 1,), dtype=np.int32)
             po = np.zeros((rows_cap + 1,), dtype=np.int32) if contours else None
             pts = np.empty((pts_cap, 2), dtype=np.int32) if contours else None
-            rc = self._retry_range(lambda: L.hvn_infer_tiles(
+            rc = self._retry_range(lambda: lib().hvn_infer_tiles(
                 self._h, n, _ptr(packed), _ptr(shapes), int(patch_in), int(batch), _ptr(pred), _ptr(inst), _ptr(table),
                 int(rows_cap), _ptr(ro), _ptr(pts), int(pts_cap if contours else 0), _ptr(po)))
-            if rc == -4:  # HVN_ERR_CAPACITY: retry with the exact size the offsets report
-                if int(ro[-1]) > rows_cap:
-                    rows_cap = int(ro[-1])
-                else:
-                    pts_cap = int(po[int(ro[-1])])
-                continue
-            check(rc)
             rows = int(ro[-1])
+            if rc == -4:
+                if rows > rows_cap:
+                    rows_cap = rows
+                else:
+                    pts_cap = int(po[rows])
+                return rc, None
             if contours:
                 po = po[: rows + 1]
                 pts = pts[: int(po[-1])]
-            return split_tiles(shapes, inst, table[:rows], ro, pred, pts, po)
-        raise HvnError(-4, "infer_tiles: capacity retries exhausted")
+            return rc, (inst, table[:rows], ro, pred, pts, po)
+        return split_tiles(shapes, *_retry_capacity("infer_tiles", attempt))
 
     def infer_tiles_begin(self, imgs, patch_in, batch=0, want_pred=True, contours=True):
         """Enqueues a tile group with hvn_infer_tiles_dev and returns at once; TilesJob.result() waits for it."""
@@ -594,19 +604,14 @@ class Context:
     def infer_tiles_dev(self, n, d_imgs, shapes, patch_in, batch, d_pred, d_inst, d_table, rows_cap, d_row_offs, d_pts,
                         pts_cap, d_pt_offs):
         """hvn_infer_tiles_dev on device pointers (shapes: host int32 [n,2]); stream-ordered, no synchronisation."""
-        L = lib()
-        L.hvn_infer_tiles_dev.argtypes = _TILES_ARGS
         sh = np.ascontiguousarray(shapes, dtype=np.int32)
-        check(L.hvn_infer_tiles_dev(self._h, int(n), _ptr(d_imgs), _ptr(sh), int(patch_in), int(batch), _ptr(d_pred),
-                                    _ptr(d_inst), _ptr(d_table), int(rows_cap), _ptr(d_row_offs), _ptr(d_pts),
-                                    int(pts_cap), _ptr(d_pt_offs)))
+        check(lib().hvn_infer_tiles_dev(self._h, int(n), _ptr(d_imgs), _ptr(sh), int(patch_in), int(batch), _ptr(d_pred),
+                                        _ptr(d_inst), _ptr(d_table), int(rows_cap), _ptr(d_row_offs), _ptr(d_pts),
+                                        int(pts_cap), _ptr(d_pt_offs)))
 
     def tile_predict_dev(self, d_img, H, W, patch_in, cell_lo, cell_hi, batch, d_pred):
-        L = lib()
-        L.hvn_tile_predict_dev.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-        check(L.hvn_tile_predict_dev(self._h, _ptr(d_img), int(H), int(W), int(patch_in), int(cell_lo), int(cell_hi),
-                                     int(batch), _ptr(d_pred)))
+        check(lib().hvn_tile_predict_dev(self._h, _ptr(d_img), int(H), int(W), int(patch_in), int(cell_lo), int(cell_hi),
+                                         int(batch), _ptr(d_pred)))
 
     def forward_postproc(self, imgs_u8, want_pred=True, max_rows=None):
         x = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
@@ -614,7 +619,9 @@ class Context:
         oh, ow, oc = self.out_shape(H, W)
         if max_rows is None:
             max_rows = max(16, oh * ow // 64)
-        while True:
+
+        def attempt():
+            nonlocal max_rows
             pred = np.empty((B, oh, ow, oc), dtype=np.float32) if want_pred else None
             inst = np.empty((B, oh, ow), dtype=np.int32)
             table = np.zeros((B, max_rows, ROW_LEN), dtype=np.int64)
@@ -623,9 +630,8 @@ class Context:
                                                                       _ptr(table), int(max_rows), _ptr(nrows)))
             if rc == -4:
                 max_rows = int(nrows.max())
-                continue
-            check(rc)
-            return pred, inst, table, nrows
+            return rc, (pred, inst, table, nrows)
+        return _retry_capacity("forward_postproc", attempt)
 
     # ---- device-pointer entry points + helpers (bench / resident pipelines)
     def malloc(self, nbytes):
@@ -675,18 +681,13 @@ class Context:
 
     def pack_tables_dev(self, d_table, d_nrows, n, max_rows, d_packed, cap_rows, d_offs):
         """padded tables [n,max_rows,10] -> packed rows [<=cap_rows,10] + offs [n+1] (all device pointers)."""
-        L = lib()
-        L.hvn_pack_tables_dev.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                                          ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
-        check(L.hvn_pack_tables_dev(self._h, _ptr(d_table), _ptr(d_nrows), int(n), int(max_rows), _ptr(d_packed),
-                                    int(cap_rows), _ptr(d_offs)))
+        check(lib().hvn_pack_tables_dev(self._h, _ptr(d_table), _ptr(d_nrows), int(n), int(max_rows), _ptr(d_packed),
+                                        int(cap_rows), _ptr(d_offs)))
 
     def stream_handle(self):
         """The context's cudaStream_t as an integer (e.g. for torch.cuda.ExternalStream)."""
         p = ctypes.c_void_p()
-        L = lib()
-        L.hvn_get_stream.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p)]
-        check(L.hvn_get_stream(self._h, ctypes.byref(p)))
+        check(lib().hvn_get_stream(self._h, ctypes.byref(p)))
         return int(p.value or 0)
 
     def forward_postproc_dev(self, d_imgs, B, H, W, d_pred, d_inst, d_table, max_rows, d_nrows):

@@ -65,6 +65,62 @@ static void use(hvn_ctx *c) {
     HVN_CUDA(cudaSetDevice(c->device));
 }
 
+// The device buffers of one call, taken from one of the context's arenas.  The call's layout declares each buffer once:
+// in() is copied from the host as it is declared, out() is copied back to the host by copy_back() (which then
+// synchronises the stream), scratch() stays on the device.  The constructor runs the layout over an ArenaSizer first,
+// so the arena is reserved for exactly the takes that follow.
+class Buffers {
+  public:
+    template <typename F> Buffers(hvn_ctx *c, Arena &a, F &&layout) : c_(c), a_(a) {
+        layout(*this);
+        a.reset();
+        a.reserve(sizer_.top);
+        sizing_ = false;
+        layout(*this);
+    }
+    template <typename T> T *scratch(size_t n) { return sizing_ ? sizer_.take<T>(n) : a_.take<T>(n); }
+    template <typename T> T *in(const T *host, size_t n) {
+        T *d = scratch<T>(n);
+        if (!sizing_) HVN_CUDA(cudaMemcpyAsync(d, host, n * sizeof(T), cudaMemcpyHostToDevice, c_->stream));
+        return d;
+    }
+    // zero: the device buffer is cleared first, so whatever the work leaves unwritten goes back as zeros
+    template <typename T> T *out(T *host, size_t n, bool zero = false) {
+        T *d = scratch<T>(n);
+        if (sizing_) return d;
+        if (zero) HVN_CUDA(cudaMemsetAsync(d, 0, n * sizeof(T), c_->stream));
+        HVN_CHECK(n_back_ < kMaxOut, HVN_ERR_INVALID, "too many staged outputs");
+        back_[n_back_++] = {host, d, n * sizeof(T)};
+        return d;
+    }
+    void copy_back() {
+        for (int i = 0; i < n_back_; ++i)
+            HVN_CUDA(cudaMemcpyAsync(back_[i].host, back_[i].dev, back_[i].bytes, cudaMemcpyDeviceToHost, c_->stream));
+        HVN_CUDA(cudaStreamSynchronize(c_->stream));
+    }
+
+  private:
+    static constexpr int kMaxOut = 8;
+    struct Out { void *host; const void *dev; size_t bytes; };
+    hvn_ctx *c_;
+    Arena &a_;
+    ArenaSizer sizer_;
+    bool sizing_ = true;
+    Out back_[kMaxOut];
+    int n_back_ = 0;
+};
+
+// Second phase of a two-phase host call, after the stream has been synchronised: `count` items of `item` bytes are
+// ready in dev.  More than `cap` is HVN_ERR_CAPACITY with the exact count; otherwise they are copied to host.  Returns
+// whether a copy was enqueued (the caller synchronises).
+static bool copy_fitting(hvn_ctx *c, void *host, const void *dev, long long count, long long cap, size_t item,
+                         const char *buffer, const char *items, const char *cap_name) {
+    HVN_CHECK(count <= cap, HVN_ERR_CAPACITY, std::string(buffer) + " too small: " + std::to_string(count) + " " + items +
+                                                  ", " + cap_name + "=" + std::to_string(cap));
+    if (count > 0) HVN_CUDA(cudaMemcpyAsync(host, dev, (size_t)count * item, cudaMemcpyDeviceToHost, c->stream));
+    return count > 0;
+}
+
 extern "C" {
 
 int hvn_abi_version(void) { return HVN_ABI_VERSION; }
@@ -248,6 +304,13 @@ static void run_postproc(hvn_ctx *c, const float *pred, int n, int H, int W, int
                                    max_rows, n_rows, c->profile >= 3 ? &c->pp_log : nullptr);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[3], c->stream));
 }
+static void run_forward_postproc(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, float *pred, int32_t *inst,
+                                 int64_t *table, int max_rows, int32_t *n_rows) {
+    int oh, ow, oc;
+    c->model->out_shape(H, W, oh, ow, oc);
+    run_forward(c, imgs, B, H, W, pred);
+    run_postproc(c, pred, B, oh, ow, oc, c->model->nr_types, inst, table, max_rows, n_rows);
+}
 static void finish_profile(hvn_ctx *c, bool cnn, bool pp) {
     if (!c->profile) return;
     HVN_CUDA(cudaStreamSynchronize(c->stream));
@@ -277,15 +340,14 @@ int hvn_forward(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, float *out
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     int oh, ow, oc;
     c->model->out_shape(H, W, oh, ow, oc);
-    size_t in_b = (size_t)B * H * W * 3, out_b = (size_t)B * oh * ow * oc * sizeof(float);
-    c->io_arena.reset();
-    c->io_arena.reserve(in_b + out_b + 1024);
-    uint8_t *d_in = c->io_arena.take<uint8_t>(in_b);
-    float *d_out = c->io_arena.take<float>(out_b / sizeof(float));
-    HVN_CUDA(cudaMemcpyAsync(d_in, imgs, in_b, cudaMemcpyHostToDevice, c->stream));
+    uint8_t *d_in;
+    float *d_out;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_in = s.in(imgs, (size_t)B * H * W * 3);
+        d_out = s.out(out, (size_t)B * oh * ow * oc);
+    });
     run_forward(c, d_in, B, H, W, d_out);
-    HVN_CUDA(cudaMemcpyAsync(out, d_out, out_b, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    io.copy_back();
     finish_profile(c, true, false);
     check_range(c);
     API_END
@@ -301,32 +363,6 @@ int hvn_postproc_dev(hvn_ctx *c, const float *pred, int n, int H, int W, int C, 
     API_END
 }
 
-int hvn_postproc(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
-                 int64_t *table, int max_rows, int32_t *n_rows) {
-    API_BEGIN
-    use(c);
-    HVN_CHECK(pred && inst && table && n_rows, HVN_ERR_INVALID, "null buffer");
-    HVN_CHECK(n >= 1 && H >= 1 && W >= 1, HVN_ERR_INVALID, "empty input");
-    size_t px = (size_t)n * H * W;
-    size_t tb = (size_t)n * max_rows * HVN_ROW_LEN;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * C * 4 + px * 4 + tb * 8 + (size_t)n * 4 + 4096);
-    float *d_pred = c->io_arena.take<float>(px * C);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int64_t *d_tab = c->io_arena.take<int64_t>(tb);
-    HVN_CUDA(cudaMemsetAsync(d_tab, 0, tb * 8, c->stream));  // rows past n_rows go back to the caller as zeros
-    int32_t *d_nr = c->io_arena.take<int32_t>(n);
-    HVN_CUDA(cudaMemcpyAsync(d_pred, pred, px * C * 4, cudaMemcpyHostToDevice, c->stream));
-    run_postproc(c, d_pred, n, H, W, C, nr_types, d_inst, d_tab, max_rows, d_nr);
-    HVN_CUDA(cudaMemcpyAsync(inst, d_inst, px * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(n_rows, d_nr, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(table, d_tab, tb * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
-    finish_profile(c, false, true);
-    check_rows(n_rows, n, max_rows);
-    API_END
-}
-
 int hvn_contours_dev(hvn_ctx *c, const int32_t *inst, const int64_t *table, const int32_t *n_rows, int n, int H, int W,
                      int max_rows, int32_t *pts, int64_t cap, int32_t *offs) {
     API_BEGIN
@@ -338,42 +374,47 @@ int hvn_contours_dev(hvn_ctx *c, const int32_t *inst, const int64_t *table, cons
     API_END
 }
 
-int hvn_postproc_contours(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
-                          int64_t *table, int max_rows, int32_t *n_rows, int32_t *pts, int64_t cap, int32_t *offs) {
+// hvn_postproc, and with `contours` hvn_postproc_contours.
+static int postproc_host(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
+                         int64_t *table, int max_rows, int32_t *n_rows, bool contours, int32_t *pts, int64_t cap,
+                         int32_t *offs) {
     API_BEGIN
     use(c);
-    HVN_CHECK(pred && inst && table && n_rows && offs && (pts || cap == 0), HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(pred && inst && table && n_rows && (!contours || (offs && (pts || cap == 0))), HVN_ERR_INVALID, "null buffer");
     HVN_CHECK(n >= 1 && H >= 1 && W >= 1 && cap >= 0, HVN_ERR_INVALID, "empty input");
-    HVN_CHECK((long long)n * max_rows < (1ll << 31), HVN_ERR_INVALID, "too many table rows");
-    size_t px = (size_t)n * H * W;
-    size_t tb = (size_t)n * max_rows * HVN_ROW_LEN;
-    size_t no = (size_t)n * max_rows + 1;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * C * 4 + px * 4 + tb * 8 + (size_t)n * 4 + no * 4 + (size_t)cap * 8 + 8192);
-    float *d_pred = c->io_arena.take<float>(px * C);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int64_t *d_tab = c->io_arena.take<int64_t>(tb);
-    HVN_CUDA(cudaMemsetAsync(d_tab, 0, tb * 8, c->stream));  // rows past n_rows go back to the caller as zeros
-    int32_t *d_nr = c->io_arena.take<int32_t>(n);
-    int32_t *d_offs = c->io_arena.take<int32_t>(no);
-    int32_t *d_pts = c->io_arena.take<int32_t>((size_t)cap * 2 + 2);
-    HVN_CUDA(cudaMemcpyAsync(d_pred, pred, px * C * 4, cudaMemcpyHostToDevice, c->stream));
+    HVN_CHECK(!contours || (long long)n * max_rows < (1ll << 31), HVN_ERR_INVALID, "too many table rows");
+    const size_t px = (size_t)n * H * W, no = (size_t)n * max_rows + 1;
+    float *d_pred;
+    int32_t *d_inst, *d_nr, *d_offs, *d_pts;
+    int64_t *d_tab;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_pred = s.in(pred, px * C);
+        d_inst = s.out(inst, px);
+        d_tab = s.out(table, (size_t)n * max_rows * HVN_ROW_LEN, true);
+        d_nr = s.out(n_rows, (size_t)n);
+        d_offs = contours ? s.out(offs, no) : nullptr;
+        d_pts = contours ? s.scratch<int32_t>((size_t)cap * 2 + 2) : nullptr;
+    });
     run_postproc(c, d_pred, n, H, W, C, nr_types, d_inst, d_tab, max_rows, d_nr);
-    c->pp_launches += contours_run(c->stream, d_inst, (const long long *)d_tab, d_nr, n, H, W, max_rows, d_pts, cap, d_offs);
-    HVN_CUDA(cudaMemcpyAsync(inst, d_inst, px * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(n_rows, d_nr, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(table, d_tab, tb * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(offs, d_offs, no * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    if (contours)
+        c->pp_launches += contours_run(c->stream, d_inst, (const long long *)d_tab, d_nr, n, H, W, max_rows, d_pts, cap,
+                                       d_offs);
+    io.copy_back();
     finish_profile(c, false, true);
     check_rows(n_rows, n, max_rows);
-    const long long total = offs[no - 1];
-    HVN_CHECK(total <= cap, HVN_ERR_CAPACITY, "contour buffer too small: " + std::to_string(total) + " points, pts_cap=" + std::to_string(cap));
-    if (total > 0) {
-        HVN_CUDA(cudaMemcpyAsync(pts, d_pts, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (contours && copy_fitting(c, pts, d_pts, offs[no - 1], cap, 8, "contour buffer", "points", "pts_cap"))
         HVN_CUDA(cudaStreamSynchronize(c->stream));
-    }
     API_END
+}
+
+int hvn_postproc(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
+                 int64_t *table, int max_rows, int32_t *n_rows) {
+    return postproc_host(c, pred, n, H, W, C, nr_types, inst, table, max_rows, n_rows, false, nullptr, 0, nullptr);
+}
+
+int hvn_postproc_contours(hvn_ctx *c, const float *pred, int n, int H, int W, int C, int nr_types, int32_t *inst,
+                          int64_t *table, int max_rows, int32_t *n_rows, int32_t *pts, int64_t cap, int32_t *offs) {
+    return postproc_host(c, pred, n, H, W, C, nr_types, inst, table, max_rows, n_rows, true, pts, cap, offs);
 }
 
 int hvn_forward_postproc_dev(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, float *pred, int32_t *inst,
@@ -385,13 +426,8 @@ int hvn_forward_postproc_dev(hvn_ctx *c, const uint8_t *imgs, int B, int H, int 
     int oh, ow, oc;
     c->model->out_shape(H, W, oh, ow, oc);
     float *d_pred = pred;
-    if (!d_pred) {
-        c->io_arena.reset();
-        c->io_arena.reserve((size_t)B * oh * ow * oc * 4 + 1024);
-        d_pred = c->io_arena.take<float>((size_t)B * oh * ow * oc);
-    }
-    run_forward(c, imgs, B, H, W, d_pred);
-    run_postproc(c, d_pred, B, oh, ow, oc, c->model->nr_types, inst, table, max_rows, n_rows);
+    if (!pred) Buffers io(c, c->io_arena, [&](Buffers &s) { d_pred = s.scratch<float>((size_t)B * oh * ow * oc); });
+    run_forward_postproc(c, imgs, B, H, W, d_pred, inst, table, max_rows, n_rows);
     finish_profile(c, true, true);
     API_END
 }
@@ -404,23 +440,20 @@ int hvn_forward_postproc(hvn_ctx *c, const uint8_t *imgs, int B, int H, int W, f
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     int oh, ow, oc;
     c->model->out_shape(H, W, oh, ow, oc);
-    size_t in_b = (size_t)B * H * W * 3, px = (size_t)B * oh * ow, tb = (size_t)B * max_rows * HVN_ROW_LEN;
-    c->io_arena.reset();
-    c->io_arena.reserve(in_b + px * oc * 4 + px * 4 + tb * 8 + (size_t)B * 4 + 8192);
-    uint8_t *d_in = c->io_arena.take<uint8_t>(in_b);
-    float *d_pred = c->io_arena.take<float>(px * oc);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int64_t *d_tab = c->io_arena.take<int64_t>(tb);
-    HVN_CUDA(cudaMemsetAsync(d_tab, 0, tb * 8, c->stream));  // rows past n_rows go back to the caller as zeros
-    int32_t *d_nr = c->io_arena.take<int32_t>(B);
-    HVN_CUDA(cudaMemcpyAsync(d_in, imgs, in_b, cudaMemcpyHostToDevice, c->stream));
-    run_forward(c, d_in, B, H, W, d_pred);
-    run_postproc(c, d_pred, B, oh, ow, oc, c->model->nr_types, d_inst, d_tab, max_rows, d_nr);
-    if (pred) HVN_CUDA(cudaMemcpyAsync(pred, d_pred, px * oc * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(inst, d_inst, px * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(n_rows, d_nr, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(table, d_tab, tb * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    const size_t px = (size_t)B * oh * ow;
+    uint8_t *d_in;
+    float *d_pred;
+    int32_t *d_inst, *d_nr;
+    int64_t *d_tab;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_in = s.in(imgs, (size_t)B * H * W * 3);
+        d_pred = pred ? s.out(pred, px * oc) : s.scratch<float>(px * oc);
+        d_inst = s.out(inst, px);
+        d_tab = s.out(table, (size_t)B * max_rows * HVN_ROW_LEN, true);
+        d_nr = s.out(n_rows, (size_t)B);
+    });
+    run_forward_postproc(c, d_in, B, H, W, d_pred, d_inst, d_tab, max_rows, d_nr);
+    io.copy_back();
     finish_profile(c, true, true);
     check_range(c);
     check_rows(n_rows, B, max_rows);
@@ -502,7 +535,7 @@ static int run_tile_predict(hvn_ctx *c, const uint8_t *imgs, const TileImage *d_
     if (batch < 1) batch = 64;
     batch = std::min(batch, 65535);
     c->tile_arena.reset();
-    c->tile_arena.reserve(tile_workspace_bytes(patch_in, oh, oc, batch) + 1024);
+    c->tile_arena.reserve(tile_workspace_bytes(patch_in, oh, oc, batch));
     return tile_predict(*c->model, c->tile_arena, c->stream, imgs, d_slots, n, lo, hi, patch_in, batch, c->chunk, pred);
 }
 
@@ -516,21 +549,22 @@ static void run_tiles(hvn_ctx *c, const TileGroup &g, const uint8_t *imgs, int p
     const int n = g.n, nt = c->model->nr_types;
     const size_t R = (size_t)g.table_rows;
     const bool contours = pt_offs != nullptr, one = n == 1;
-    // a group of one writes its table and its point counts in place (the packing is the identity)
-    const size_t ws = (size_t)n * sizeof(TileImage) + (size_t)n * 8 + (one ? 0 : R * 80) + (contours && !one ? R * 4 : 0) +
-                      (pred ? 0 : g.px * g.oc * 4) + (inst ? 0 : g.px * 4) + 8 * 256;
     c->group_table_rows = one ? 0 : (long long)R;
-    c->group_arena.reset();
-    c->group_arena.reserve(ws);
-    TileImage *d_slots = c->group_arena.take<TileImage>(n);
-    int *d_slot_of = c->group_arena.take<int>(n);
-    int *d_nrows = c->group_arena.take<int>(n);
-    long long *pad = one ? (long long *)table : c->group_arena.take<long long>(R * 10);
-    int *cnt = !contours ? nullptr : (one ? pt_offs : c->group_arena.take<int>(R));
-    if (!pred) pred = c->group_arena.take<float>(g.px * g.oc);
-    if (!inst) inst = c->group_arena.take<int32_t>(g.px);
-    *pred_out = pred;
-    *inst_out = inst;
+    TileImage *d_slots;
+    int *d_slot_of, *d_nrows, *cnt;
+    long long *pad;
+    // a group of one writes its table and its point counts in place (the packing is the identity)
+    Buffers ws(c, c->group_arena, [&](Buffers &b) {
+        d_slots = b.scratch<TileImage>(n);
+        d_slot_of = b.scratch<int>(n);
+        d_nrows = b.scratch<int>(n);
+        pad = one ? (long long *)table : b.scratch<long long>(R * 10);
+        cnt = !contours ? nullptr : (one ? pt_offs : b.scratch<int>(R));
+        *pred_out = pred ? pred : b.scratch<float>(g.px * g.oc);
+        *inst_out = inst ? inst : b.scratch<int32_t>(g.px);
+    });
+    pred = *pred_out;
+    inst = *inst_out;
     upload_slots(c, g, d_slots, d_slot_of);
 
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
@@ -599,9 +633,8 @@ int hvn_tile_predict_dev(hvn_ctx *c, const uint8_t *img, int H, int W, int patch
     TileGroup g;
     plan_tiles(c, 1, shape, patch_in, 1, g);
     HVN_CHECK(cell_lo >= 0 && cell_hi <= g.cells && cell_lo <= cell_hi, -1, "patch range outside the grid");
-    c->group_arena.reset();
-    c->group_arena.reserve(1024);
-    TileImage *d_slots = c->group_arena.take<TileImage>(1);
+    TileImage *d_slots;
+    Buffers ws(c, c->group_arena, [&](Buffers &b) { d_slots = b.scratch<TileImage>(1); });
     upload_slots(c, g, d_slots, nullptr);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[0], c->stream));
     c->model->kernel_launches += run_tile_predict(c, img, d_slots, 1, cell_lo, cell_hi, patch_in, batch, pred);
@@ -620,42 +653,30 @@ int hvn_infer_tile(hvn_ctx *c, const uint8_t *img, int H, int W, int patch_in, i
     const int32_t shape[2] = {H, W};
     TileGroup g;
     plan_tiles(c, 1, shape, patch_in, max_rows, g);
-    const int oc = g.oc;
-    const size_t px = (size_t)H * W, tb = (size_t)max_rows * HVN_ROW_LEN, no = (size_t)max_rows + 1;
+    const size_t px = (size_t)H * W;
     if (!offs) cap = 0;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 3 + px * oc * 4 + px * 4 + tb * 8 + no * 4 + (size_t)cap * 8 + 16384);
-    uint8_t *d_img = c->io_arena.take<uint8_t>(px * 3);
-    float *d_pred = c->io_arena.take<float>(px * oc);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int64_t *d_tab = c->io_arena.take<int64_t>(tb);
-    HVN_CUDA(cudaMemsetAsync(d_tab, 0, tb * 8, c->stream));  // rows past n_rows go back to the caller as zeros
-    int32_t *d_ro = c->io_arena.take<int32_t>(2);
-    int32_t *d_offs = offs ? c->io_arena.take<int32_t>(no) : nullptr;
-    int32_t *d_pts = c->io_arena.take<int32_t>((size_t)cap * 2 + 2);
-    HVN_CUDA(cudaMemcpyAsync(d_img, img, px * 3, cudaMemcpyHostToDevice, c->stream));
-    float *wp;
-    int32_t *wi;
-    run_tiles(c, g, d_img, patch_in, batch, d_pred, d_inst, d_tab, max_rows, d_ro, d_pts, cap, d_offs, &wp, &wi);
     int32_t ro[2] = {0, 0};
-    if (pred) HVN_CUDA(cudaMemcpyAsync(pred, d_pred, px * oc * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(inst, d_inst, px * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(ro, d_ro, 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(table, d_tab, tb * 8, cudaMemcpyDeviceToHost, c->stream));
-    if (offs) HVN_CUDA(cudaMemcpyAsync(offs, d_offs, no * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    uint8_t *d_img;
+    float *d_pred, *wp;
+    int32_t *d_inst, *d_ro, *d_offs, *d_pts, *wi;
+    int64_t *d_tab;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_img = s.in(img, px * 3);
+        d_pred = pred ? s.out(pred, px * g.oc) : s.scratch<float>(px * g.oc);
+        d_inst = s.out(inst, px);
+        d_tab = s.out(table, (size_t)max_rows * HVN_ROW_LEN, true);
+        d_ro = s.out(ro, 2);
+        d_offs = offs ? s.out(offs, (size_t)max_rows + 1) : nullptr;
+        d_pts = s.scratch<int32_t>((size_t)cap * 2 + 2);
+    });
+    run_tiles(c, g, d_img, patch_in, batch, d_pred, d_inst, d_tab, max_rows, d_ro, d_pts, cap, d_offs, &wp, &wi);
+    io.copy_back();
     finish_profile(c, true, true);
     check_range(c);
     n_rows[0] = ro[1];
     check_rows(n_rows, 1, max_rows);
-    if (offs) {
-        const long long total = offs[no - 1];
-        HVN_CHECK(total <= cap, HVN_ERR_CAPACITY, "contour buffer too small: " + std::to_string(total) + " points, pts_cap=" + std::to_string(cap));
-        if (total > 0) {
-            HVN_CUDA(cudaMemcpyAsync(pts, d_pts, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
-            HVN_CUDA(cudaStreamSynchronize(c->stream));
-        }
-    }
+    if (offs && copy_fitting(c, pts, d_pts, offs[max_rows], cap, 8, "contour buffer", "points", "pts_cap"))
+        HVN_CUDA(cudaStreamSynchronize(c->stream));
     API_END
 }
 
@@ -668,38 +689,29 @@ int hvn_infer_tiles(hvn_ctx *c, int n, const uint8_t *imgs, const int32_t *shape
     TileGroup g;
     plan_tiles(c, n, shapes, patch_in, rows_cap, g);
     if (!pt_offs) pts_cap = 0;
-    const size_t px = g.px, no = pt_offs ? (size_t)rows_cap + 1 : 0;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 3 + px * g.oc * 4 + px * 4 + (size_t)rows_cap * 80 + (size_t)(n + 1) * 4 + no * 4 +
-                        (size_t)pts_cap * 8 + 16384);
-    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
-    float *d_pred = c->io_arena.take<float>(px * g.oc);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int64_t *d_tab = c->io_arena.take<int64_t>((size_t)rows_cap * HVN_ROW_LEN);
-    int32_t *d_ro = c->io_arena.take<int32_t>((size_t)n + 1);
-    int32_t *d_po = pt_offs ? c->io_arena.take<int32_t>(no) : nullptr;
-    int32_t *d_pts = c->io_arena.take<int32_t>((size_t)pts_cap * 2 + 2);
-    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
-    float *wp;
-    int32_t *wi;
+    const size_t px = g.px;
+    uint8_t *d_imgs;
+    float *d_pred, *wp;
+    int32_t *d_inst, *d_ro, *d_po, *d_pts, *wi;
+    int64_t *d_tab;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_imgs = s.in(imgs, px * 3);
+        d_pred = s.scratch<float>(px * g.oc);
+        d_inst = s.scratch<int32_t>(px);
+        d_tab = s.scratch<int64_t>((size_t)rows_cap * HVN_ROW_LEN);
+        d_ro = s.out(row_offs, (size_t)n + 1);
+        d_po = pt_offs ? s.out(pt_offs, (size_t)rows_cap + 1) : nullptr;
+        d_pts = s.scratch<int32_t>((size_t)pts_cap * 2 + 2);
+    });
     run_tiles(c, g, d_imgs, patch_in, batch, d_pred, d_inst, d_tab, rows_cap, d_ro, d_pts, pts_cap, d_po, &wp, &wi);
     if (pred) copy_maps(c, g, pred, d_pred, (size_t)g.oc * 4, cudaMemcpyDeviceToHost);
     copy_maps(c, g, inst, d_inst, 4, cudaMemcpyDeviceToHost);
-    HVN_CUDA(cudaMemcpyAsync(row_offs, d_ro, (size_t)(n + 1) * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (pt_offs) HVN_CUDA(cudaMemcpyAsync(pt_offs, d_po, no * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    io.copy_back();
     finish_profile(c, true, true);
     check_range(c);
     const long long rows = row_offs[n];
-    HVN_CHECK(rows <= rows_cap, HVN_ERR_CAPACITY,
-              "instance table too small: " + std::to_string(rows) + " rows, rows_cap=" + std::to_string(rows_cap));
-    if (rows > 0) HVN_CUDA(cudaMemcpyAsync(table, d_tab, (size_t)rows * 80, cudaMemcpyDeviceToHost, c->stream));
-    if (pt_offs) {
-        const long long total = pt_offs[rows];
-        HVN_CHECK(total <= pts_cap, HVN_ERR_CAPACITY,
-                  "contour buffer too small: " + std::to_string(total) + " points, pts_cap=" + std::to_string(pts_cap));
-        if (total > 0) HVN_CUDA(cudaMemcpyAsync(pts, d_pts, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
-    }
+    copy_fitting(c, table, d_tab, rows, rows_cap, HVN_ROW_LEN * 8, "instance table", "rows", "rows_cap");
+    if (pt_offs) copy_fitting(c, pts, d_pts, pt_offs[rows], pts_cap, 8, "contour buffer", "points", "pts_cap");
     HVN_CUDA(cudaStreamSynchronize(c->stream));
     API_END
 }
@@ -760,31 +772,28 @@ int hvn_inst_pairs(hvn_ctx *c, const int32_t *tru, const int32_t *pred, int n, i
     use(c);
     check_pairs_args(tru, pairs, cap, offs, n, H, W);
     const size_t px = (size_t)n * H * W;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 4 * (pred ? 2 : 1) + (size_t)(n + 1) * 8 + 4096);
-    int32_t *d_t = c->io_arena.take<int32_t>(px);
-    int32_t *d_p = pred ? c->io_arena.take<int32_t>(px) : nullptr;
-    long long *d_offs = c->io_arena.take<long long>((size_t)n + 1);
-    HVN_CUDA(cudaMemcpyAsync(d_t, tru, px * 4, cudaMemcpyHostToDevice, c->stream));
-    if (pred) HVN_CUDA(cudaMemcpyAsync(d_p, pred, px * 4, cudaMemcpyHostToDevice, c->stream));
+    long long *h_offs = (long long *)offs, *d_offs, *d_pairs;
+    int32_t *d_t, *d_p;
+    Buffers maps(c, c->io_arena, [&](Buffers &s) {
+        d_t = s.in(tru, px);
+        d_p = pred ? s.in(pred, px) : nullptr;
+        d_offs = s.out(h_offs, (size_t)n + 1);
+    });
     PairWork w;
     inst_pairs_count(c->stats_arena, c->stream, d_t, d_p, n, H, W, d_offs, w);
     int err = 0;
     HVN_CUDA(cudaMemcpyAsync(&err, w.err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(offs, d_offs, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    maps.copy_back();
     const long long total = offs[n];
     check_pairs_result(err, total, cap);
     if (total == 0) return HVN_OK;
     // the maps are no longer needed: the staging arena now holds the rows
-    c->io_arena.reset();
-    c->io_arena.reserve((size_t)total * 24 + (size_t)(n + 1) * 8 + 1024);
-    long long *d_pairs = c->io_arena.take<long long>((size_t)total * 3);
-    w.offs = c->io_arena.take<long long>((size_t)n + 1);
-    HVN_CUDA(cudaMemcpyAsync(w.offs, offs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    Buffers rows(c, c->io_arena, [&](Buffers &s) {
+        d_pairs = s.out((long long *)pairs, (size_t)total * 3);
+        w.offs = s.in(h_offs, (size_t)n + 1);
+    });
     inst_pairs_emit(c->stream, w, d_pairs, total);
-    HVN_CUDA(cudaMemcpyAsync(pairs, d_pairs, (size_t)total * 24, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    rows.copy_back();
     API_END
 }
 
@@ -827,172 +836,132 @@ int hvn_targets(hvn_ctx *c, const int32_t *inst, int n, int H, int W, int crop_h
     HVN_CHECK(inst && hv && flags, HVN_ERR_INVALID, "null buffer");
     check_targets_args(n, H, W, crop_h, crop_w);
     const size_t px = (size_t)n * H * W;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 12 + (size_t)n * 4 + 4096);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    float *d_hv = c->io_arena.take<float>(px * 2);
-    int32_t *d_flags = c->io_arena.take<int32_t>(n);
-    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
+    int32_t *d_inst, *d_flags;
+    float *d_hv;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_inst = s.in(inst, px);
+        d_hv = s.out(hv, px * 2);
+        d_flags = s.out(flags, (size_t)n);
+    });
     TargetWork w;
     targets_run(c->targets_arena, c->stream, d_inst, n, H, W, crop_h, crop_w, d_hv, d_flags, w);
-    HVN_CUDA(cudaMemcpyAsync(hv, d_hv, px * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    io.copy_back();
     check_targets_result(w);
     API_END
 }
 
-// Forward, targets and counts of one batch, enqueued on the context stream; the caller synchronises and checks.
+// Forward, targets and the reduction of one validation batch, enqueued on the context stream.  Without `loss`
+// (hvn_valid): the plain head and the counts.  With it (hvn_valid_loss): the full head, the loss sums and the counts;
+// probs (may be null) receives the [B,h,w,4+nt] probabilities by a copy of kind pk.  The caller synchronises and calls
+// finish_valid.
 static void run_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
-                      int64_t *counts, double *sse, int32_t *flags, TargetWork &w) {
+                      int64_t *counts, double *sse, int32_t *flags, bool loss, double *sums, float *probs,
+                      cudaMemcpyKind pk, TargetWork &w, LossWork &lw) {
     HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
     const int nt = c->model->nr_types;
-    HVN_CHECK(imgs && inst && counts && sse && flags, HVN_ERR_INVALID, "null buffer");
+    HVN_CHECK(imgs && inst && counts && sse && flags && (sums || !loss), HVN_ERR_INVALID, "null buffer");
     HVN_CHECK(nt == 0 || type, HVN_ERR_INVALID, "a model with nr_types > 0 needs a type map");
     int oh, ow, oc;
     c->model->out_shape(H, W, oh, ow, oc);
     check_targets_args(B, H, W, oh, ow);
+    if (loss) oc = nt + 4;
     const size_t opx = (size_t)B * oh * ow, px = (size_t)B * H * W;
-    c->valid_arena.reset();
-    c->valid_arena.reserve(opx * oc * 4 + px * 8 + 1024);
-    float *d_pred = c->valid_arena.take<float>(opx * oc);
-    float *d_hv = c->valid_arena.take<float>(px * 2);
+    float *d_pred, *d_hv;
+    Buffers ws(c, c->valid_arena, [&](Buffers &b) {
+        d_pred = b.scratch<float>(opx * oc);
+        d_hv = b.scratch<float>(px * 2);
+    });
     HVN_CUDA(cudaMemsetAsync(counts, 0, (size_t)(3 + 2 * nt) * 8, c->stream));
-    HVN_CUDA(cudaMemsetAsync(sse, 0, sizeof(double), c->stream));
-    run_forward(c, imgs, B, H, W, d_pred);
-    targets_run(c->targets_arena, c->stream, inst, B, H, W, oh, ow, d_hv, flags, w);
-    valid_reduce(c->stream, d_pred, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, oc, nt, (long long *)counts, sse);
-}
-
-int hvn_valid_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
-                  int64_t *counts, double *sse, int32_t *flags) {
-    API_BEGIN
-    use(c);
-    TargetWork w;
-    run_valid(c, imgs, inst, type, B, H, W, counts, sse, flags, w);
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
-    finish_profile(c, true, false);
-    check_range(c);
-    check_targets_result(w);
-    API_END
-}
-
-int hvn_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
-              int64_t *counts, double *sse, int32_t *flags) {
-    API_BEGIN
-    use(c);
-    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
-    HVN_CHECK(imgs && inst && counts && sse && flags, HVN_ERR_INVALID, "null buffer");
-    check_targets_args(B, H, W, 1, 1);
-    const int nt = c->model->nr_types;
-    const size_t px = (size_t)B * H * W, nc = 3 + 2 * (size_t)nt;
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 3 + px * 4 * (nt ? 2 : 1) + nc * 8 + (size_t)B * 4 + 8 + 4096);
-    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int32_t *d_type = nt && type ? c->io_arena.take<int32_t>(px) : nullptr;
-    int64_t *d_counts = c->io_arena.take<int64_t>(nc);
-    double *d_sse = c->io_arena.take<double>(1);
-    int32_t *d_flags = c->io_arena.take<int32_t>(B);
-    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
-    if (d_type) HVN_CUDA(cudaMemcpyAsync(d_type, type, px * 4, cudaMemcpyHostToDevice, c->stream));
-    TargetWork w;
-    run_valid(c, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags, w);
-    HVN_CUDA(cudaMemcpyAsync(counts, d_counts, nc * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(sse, d_sse, 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
-    finish_profile(c, true, false);
-    check_range(c);
-    check_targets_result(w);
-    API_END
-}
-
-// Forward with every probability, targets, loss sums and counts of one batch, enqueued on the context stream; the
-// caller synchronises and checks.  probs (may be null) receives the [B,h,w,4+nt] map by a copy of kind pk.
-static void run_valid_loss(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H,
-                           int W, int64_t *counts, double *sse, double *sums, float *probs, cudaMemcpyKind pk,
-                           int32_t *flags, TargetWork &w, LossWork &lw) {
-    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
-    const int nt = c->model->nr_types;
-    HVN_CHECK(imgs && inst && counts && sse && sums && flags, HVN_ERR_INVALID, "null buffer");
-    HVN_CHECK(nt == 0 || type, HVN_ERR_INVALID, "a model with nr_types > 0 needs a type map");
-    int oh, ow, oc;
-    c->model->out_shape(H, W, oh, ow, oc);
-    check_targets_args(B, H, W, oh, ow);
-    oc = nt + 4;
-    const size_t opx = (size_t)B * oh * ow, px = (size_t)B * H * W;
-    c->valid_arena.reset();
-    c->valid_arena.reserve(opx * oc * 4 + px * 8 + 1024);
-    float *d_probs = c->valid_arena.take<float>(opx * oc);
-    float *d_hv = c->valid_arena.take<float>(px * 2);
-    HVN_CUDA(cudaMemsetAsync(counts, 0, (size_t)(3 + 2 * nt) * 8, c->stream));
-    run_forward(c, imgs, B, H, W, d_probs, OUT_FULL);
+    if (!loss) {
+        HVN_CUDA(cudaMemsetAsync(sse, 0, sizeof(double), c->stream));
+        run_forward(c, imgs, B, H, W, d_pred);
+        targets_run(c->targets_arena, c->stream, inst, B, H, W, oh, ow, d_hv, flags, w);
+        valid_reduce(c->stream, d_pred, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, oc, nt, (long long *)counts, sse);
+        return;
+    }
+    run_forward(c, imgs, B, H, W, d_pred, OUT_FULL);
     targets_run(c->targets_arena, c->stream, inst, B, H, W, oh, ow, d_hv, flags, w);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[2], c->stream));
-    loss_reduce(c->loss_arena, c->stream, d_probs, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, nt, sums,
+    loss_reduce(c->loss_arena, c->stream, d_pred, inst, nt ? type : nullptr, d_hv, B, H, W, oh, ow, nt, sums,
                 (long long *)counts, lw);
     if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[3], c->stream));
     HVN_CUDA(cudaMemcpyAsync(sse, sums + LS_HV_SQ, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-    if (probs) HVN_CUDA(cudaMemcpyAsync(probs, d_probs, opx * oc * 4, pk, c->stream));
+    if (probs) HVN_CUDA(cudaMemcpyAsync(probs, d_pred, opx * oc * 4, pk, c->stream));
 }
 // After the context stream has been synchronised.
-static void finish_valid_loss(hvn_ctx *c, const TargetWork &w, const LossWork &lw) {
+static void finish_valid(hvn_ctx *c, bool loss, const TargetWork &w, const LossWork &lw) {
     finish_profile(c, true, false);
-    if (c->profile) HVN_CUDA(cudaEventElapsedTime(&c->ms_loss, c->ev[2], c->ev[3]));
+    if (loss && c->profile) HVN_CUDA(cudaEventElapsedTime(&c->ms_loss, c->ev[2], c->ev[3]));
     check_range(c);
     check_targets_result(w);
+    if (!loss) return;
     int err = 0;
     HVN_CUDA(cudaMemcpy(&err, lw.err, sizeof(int), cudaMemcpyDeviceToHost));
     HVN_CHECK(!err, HVN_ERR_INVALID,
               "type id outside 0.." + std::to_string(c->model->nr_types - 1) + " inside the output crop");
 }
 
-int hvn_valid_loss_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
-                       int64_t *counts, double *sse, int32_t *flags, double *sums, float *probs) {
+static int valid_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                     int64_t *counts, double *sse, int32_t *flags, bool loss, double *sums, float *probs) {
     API_BEGIN
     use(c);
     TargetWork w;
     LossWork lw;
-    run_valid_loss(c, imgs, inst, type, B, H, W, counts, sse, sums, probs, cudaMemcpyDeviceToDevice, flags, w, lw);
+    run_valid(c, imgs, inst, type, B, H, W, counts, sse, flags, loss, sums, probs, cudaMemcpyDeviceToDevice, w, lw);
     HVN_CUDA(cudaStreamSynchronize(c->stream));
-    finish_valid_loss(c, w, lw);
+    finish_valid(c, loss, w, lw);
     API_END
+}
+
+static int valid_host(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                      int64_t *counts, double *sse, int32_t *flags, bool loss, double *sums, float *probs) {
+    API_BEGIN
+    use(c);
+    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
+    HVN_CHECK(imgs && inst && counts && sse && flags && (sums || !loss), HVN_ERR_INVALID, "null buffer");
+    check_targets_args(B, H, W, 1, 1);
+    const int nt = c->model->nr_types;
+    const size_t px = (size_t)B * H * W;
+    uint8_t *d_imgs;
+    int32_t *d_inst, *d_type, *d_flags;
+    int64_t *d_counts;
+    double *d_sse, *d_sums;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_imgs = s.in(imgs, px * 3);
+        d_inst = s.in(inst, px);
+        d_type = nt && type ? s.in(type, px) : nullptr;
+        d_counts = s.out(counts, 3 + 2 * (size_t)nt);
+        d_sse = s.out(sse, 1);
+        d_sums = loss ? s.out(sums, (size_t)loss_nsums(nt)) : nullptr;
+        d_flags = s.out(flags, (size_t)B);
+    });
+    TargetWork w;
+    LossWork lw;
+    run_valid(c, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_flags, loss, d_sums, probs, cudaMemcpyDeviceToHost,
+              w, lw);
+    io.copy_back();
+    finish_valid(c, loss, w, lw);
+    API_END
+}
+
+int hvn_valid_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                  int64_t *counts, double *sse, int32_t *flags) {
+    return valid_dev(c, imgs, inst, type, B, H, W, counts, sse, flags, false, nullptr, nullptr);
+}
+
+int hvn_valid(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+              int64_t *counts, double *sse, int32_t *flags) {
+    return valid_host(c, imgs, inst, type, B, H, W, counts, sse, flags, false, nullptr, nullptr);
+}
+
+int hvn_valid_loss_dev(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
+                       int64_t *counts, double *sse, int32_t *flags, double *sums, float *probs) {
+    return valid_dev(c, imgs, inst, type, B, H, W, counts, sse, flags, true, sums, probs);
 }
 
 int hvn_valid_loss(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const int32_t *type, int B, int H, int W,
                    int64_t *counts, double *sse, int32_t *flags, double *sums, float *probs) {
-    API_BEGIN
-    use(c);
-    HVN_CHECK(c->model, HVN_ERR_STATE, "context has no model");
-    HVN_CHECK(imgs && inst && counts && sse && flags && sums, HVN_ERR_INVALID, "null buffer");
-    check_targets_args(B, H, W, 1, 1);
-    const int nt = c->model->nr_types;
-    const size_t px = (size_t)B * H * W, nc = 3 + 2 * (size_t)nt, ns = loss_nsums(nt);
-    c->io_arena.reset();
-    c->io_arena.reserve(px * 3 + px * 4 * (nt ? 2 : 1) + (nc + 1 + ns) * 8 + (size_t)B * 4 + 8 + 4096);
-    uint8_t *d_imgs = c->io_arena.take<uint8_t>(px * 3);
-    int32_t *d_inst = c->io_arena.take<int32_t>(px);
-    int32_t *d_type = nt && type ? c->io_arena.take<int32_t>(px) : nullptr;
-    int64_t *d_counts = c->io_arena.take<int64_t>(nc);
-    double *d_sse = c->io_arena.take<double>(1);
-    double *d_sums = c->io_arena.take<double>(ns);
-    int32_t *d_flags = c->io_arena.take<int32_t>(B);
-    HVN_CUDA(cudaMemcpyAsync(d_imgs, imgs, px * 3, cudaMemcpyHostToDevice, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(d_inst, inst, px * 4, cudaMemcpyHostToDevice, c->stream));
-    if (d_type) HVN_CUDA(cudaMemcpyAsync(d_type, type, px * 4, cudaMemcpyHostToDevice, c->stream));
-    TargetWork w;
-    LossWork lw;
-    run_valid_loss(c, d_imgs, d_inst, d_type, B, H, W, d_counts, d_sse, d_sums, probs, cudaMemcpyDeviceToHost, d_flags,
-                   w, lw);
-    HVN_CUDA(cudaMemcpyAsync(counts, d_counts, nc * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(sse, d_sse, 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(sums, d_sums, ns * 8, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaMemcpyAsync(flags, d_flags, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
-    HVN_CUDA(cudaStreamSynchronize(c->stream));
-    finish_valid_loss(c, w, lw);
-    API_END
+    return valid_host(c, imgs, inst, type, B, H, W, counts, sse, flags, true, sums, probs);
 }
 
 // ---------------------------------------------------------------------------------------------------

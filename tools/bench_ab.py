@@ -8,8 +8,9 @@
 
 `run` runs `bench.py --gpus 1` from both trees in one process tree, alternating them (base first in even rounds, the
 working tree first in odd ones) so that clock drift and neighbours on the host hit both alike.  It writes
-DIR/bench_ab.json with, per workload, every round's `value` for both trees, their medians, their spread
-((max - min) / median) and the ratio of the medians; the card's name, power limit and max SM clock, read by nvidia-smi in
+DIR/bench_ab.json with, per workload, every round's `value` and `e2e.value` (the host-buffer entry point) for both
+trees, their medians, their spread ((max - min) / median) and the ratios of the medians, and each tree's e2e
+`h2d_bytes_per_step` / `d2h_bytes_per_step`; the card's name, power limit and max SM clock, read by nvidia-smi in
 the same run; and whether both trees' `--dump-outputs` (written to a temporary directory, removed afterwards) are
 bit-identical:
 * orig256 and fast64 in precision "highest" (the dump of the first timed round: it is written after the timed steps);
@@ -106,19 +107,25 @@ def run(args):
     dumps = tempfile.mkdtemp(prefix="bench_ab_")   # output dumps: compared here, then removed
     for spec in args.rounds.split(","):
         wl, n = spec.split("=")
-        vals = {"base": [], "this": []}
+        vals, e2e, copies = {"base": [], "this": []}, {"base": [], "this": []}, {}
         for r in range(int(n)):
             for t in (("base", "this") if r % 2 == 0 else ("this", "base")):
                 dump = os.path.join(dumps, t, wl + "_highest") if r == 0 and wl in ("orig256", "fast64") else None
                 line = _bench(trees[t], wl, args.steps, args.warmup, dump=dump)
                 vals[t].append(line["value"])
+                e2e[t].append(line["e2e"]["value"])
+                copies[t] = {k: line["e2e"].get(k) for k in ("h2d_bytes_per_step", "d2h_bytes_per_step")}
                 print("%s round %d %s: %.3f %s" % (wl, r, t, line["value"], line["unit"]), flush=True)
         w = {t: _stats(v) for t, v in vals.items()}
         w["ratio"] = w["this"]["median"] / w["base"]["median"]
         w["unit"] = line["unit"]
+        w["e2e"] = {t: _stats(v) for t, v in e2e.items()}
+        w["e2e"]["ratio"] = w["e2e"]["this"]["median"] / w["e2e"]["base"]["median"]
+        w["e2e"]["copies"] = copies
         res["workloads"][wl] = w
-        print("%s: this / base = %.4f (spread base %.2f %%, this %.2f %%)" % (
-            wl, w["ratio"], 100 * w["base"]["spread"], 100 * w["this"]["spread"]), flush=True)
+        for tag, x in (("value", w), ("e2e", w["e2e"])):
+            print("%s %s: this / base = %.4f (spread base %.2f %%, this %.2f %%)" % (
+                wl, tag, x["ratio"], 100 * x["base"]["spread"], 100 * x["this"]["spread"]), flush=True)
     for wl in ("orig256", "fast64"):
         for t in ("base", "this"):
             _bench(trees[t], wl, 1, 1, extra=["--opt", "precision=1"], dump=os.path.join(dumps, t, wl + "_high"))
