@@ -10,6 +10,11 @@ LIB_PATH = os.path.join(_HERE, "libhvn.so")
 ROW_LEN = 10
 # hvn_targets flag bits (include/hvn.h HVN_TG_*): the maps the reference's gen_instance_hv_map raises ValueError on
 TG_NO_BACKGROUND, TG_NO_BACKGROUND_CROP, TG_EMPTY_BOX = 1, 2, 4
+# columns of hvn_inst_features (include/hvn.h HVN_FEAT_*), in order
+FEATURE_NAMES = ("area", "contour_area", "perimeter", "convex_area", "solidity", "circularity", "major_axis_length",
+                 "minor_axis_length", "eccentricity", "orientation", "feret_max", "mean_r", "mean_g", "mean_b", "std_r",
+                 "std_g", "std_b", "np_prob_mean")
+FEAT_LEN = len(FEATURE_NAMES)
 _lib = None
 
 
@@ -24,6 +29,7 @@ class HvnError(RuntimeError):
 _P, _S, _I, _I64, _SZ = ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t
 _VALID = [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P]
 _TILES_ARGS = [_P, _I, _P, _P, _I, _I, _P, _P, _P, _I64, _P, _P, _I64, _P]
+_FEAT_ARGS = [_P, _I, _P, _P, _P, _P, _I, _P, _P, _I64, _P, _P, _P]
 PROTOTYPES = {
     "hvn_abi_version": (_I, []),
     "hvn_last_error": (_S, []),
@@ -61,6 +67,8 @@ PROTOTYPES = {
     "hvn_valid_dev": (_I, _VALID),
     "hvn_valid_loss": (_I, _VALID + [_P, _P]),
     "hvn_valid_loss_dev": (_I, _VALID + [_P, _P]),
+    "hvn_inst_features": (_I, _FEAT_ARGS),
+    "hvn_inst_features_dev": (_I, _FEAT_ARGS),
     "hvn_malloc": (_I, [_P, _SZ, _P]),
     "hvn_free": (_I, [_P, _P]),
     "hvn_malloc_host": (_I, [_P, _SZ, _P]),
@@ -161,9 +169,10 @@ def tiles_sizes(shapes):
     return sum(max(16, p // 64) for p in px), sum(max(4096, p // 16) for p in px)
 
 
-def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None):
+def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None, feats=None):
     """Packed outputs of hvn_infer_tiles -> one (pred [H,W,C] or None, inst [H,W], table [k,10], offs [k+1], pts [m,2]
-    or None) per image, the tuple Context.infer_tile returns: offs index the image's own points."""
+    or None) per image, the tuple Context.infer_tile returns: offs index the image's own points.  With feats (the
+    group's hvn_inst_features rows [rows,FEAT_LEN]) each tuple gains the image's rows of it."""
     out = []
     p0 = 0
     C = None if pred is None else pred.size // max(1, int(sum(int(h) * int(w) for h, w in shapes)))
@@ -176,7 +185,7 @@ def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None
         if pt_offs is not None:
             offs = np.asarray(pt_offs[r0:r1 + 1], dtype=np.int64) - int(pt_offs[r0])
             pt = pts[int(pt_offs[r0]):int(pt_offs[r1])]
-        out.append((pm, im, table[r0:r1], offs, pt))
+        out.append((pm, im, table[r0:r1], offs, pt) + (() if feats is None else (feats[r0:r1],)))
         p0 += h * w
     return out
 
@@ -184,17 +193,28 @@ def split_tiles(shapes, inst, table, row_offs, pred=None, pts=None, pt_offs=None
 class TilesJob:
     """A tile group enqueued with hvn_infer_tiles_dev (Context.infer_tiles_begin).  result() synchronises and returns
     what Context.infer_tiles returns.  A capacity failure reruns the group through Context.infer_tiles with the sizes the
-    offsets report; a range failure reruns it there too, which raises act_shift."""
+    offsets report; a range failure reruns it there too, which raises act_shift.  With features, result() measures
+    every instance (hvn_inst_features_dev) on the group's device image, instance and prediction maps before they are
+    freed; the prediction map is kept on the device for that even when it is not wanted back.  Such a group is rerun
+    as another TilesJob (the maps are measured on the device there too): with the reported sizes after a capacity
+    failure, with act_shift raised by 6 after a range failure, as Context._retry_range does."""
 
-    def __init__(self, ctx, imgs, patch_in, batch, want_pred, contours):
+    MAX_RERUNS = 9  # two capacity growths and six act_shift steps, and one to spare
+
+    def __init__(self, ctx, imgs, patch_in, batch, want_pred, contours, features=False, rows_cap=None, pts_cap=None,
+                 reruns=0):
+        if features and not contours:
+            raise ValueError("instance features need the contours")
         self.ctx, self.imgs, self.patch_in, self.batch = ctx, imgs, patch_in, batch
-        self.want_pred, self.contours = want_pred, contours
+        self.want_pred, self.contours, self.features, self.reruns = want_pred, contours, features, reruns
         self.packed, self.shapes = pack_images(imgs)
         n = self.shapes.shape[0]
         px = int(self.packed.size // 3)
         self.oc = ctx.out_shape(patch_in, patch_in)[2]
-        self.rows_cap, self.pts_cap = tiles_sizes(self.shapes)
-        sizes = {"img": px * 3, "pred": px * self.oc * 4 if want_pred else 0, "inst": px * 4,
+        r0, p0 = tiles_sizes(self.shapes)
+        self.rows_cap = r0 if rows_cap is None else int(rows_cap)
+        self.pts_cap = p0 if pts_cap is None else int(pts_cap)
+        sizes = {"img": px * 3, "pred": px * self.oc * 4 if want_pred or features else 0, "inst": px * 4,
                  "table": self.rows_cap * ROW_LEN * 8, "ro": (n + 1) * 4,
                  "po": (self.rows_cap + 1) * 4 if contours else 0, "pts": self.pts_cap * 8 if contours else 0}
         self.d = {k: (ctx.malloc(b) if b else None) for k, b in sizes.items()}
@@ -222,7 +242,7 @@ class TilesJob:
             except HvnError as e:
                 if e.code != -6:
                     raise
-                return self._rerun()
+                return self._rerun(range_failed=True)
             ro = np.zeros((n + 1,), dtype=np.int32)
             ctx.d2h(ro, self.d["ro"], ro.nbytes)
             rows = int(ro[-1])
@@ -250,16 +270,36 @@ class TilesJob:
                 if pts.size:
                     ctx.d2h(pts, self.d["pts"], pts.nbytes)
                 po = po[: rows + 1]
+            feats = None
+            if self.features:
+                feats = np.empty((rows, FEAT_LEN), dtype=np.float64)
+                d_feats = ctx.malloc(max(1, feats.nbytes))
+                try:
+                    ctx.inst_features_dev(n, self.shapes, self.d["inst"], self.d["img"], self.d["pred"], self.oc,
+                                          self.d["table"], self.d["ro"], rows, self.d["pts"], self.d["po"], d_feats)
+                    if rows:
+                        ctx.d2h(feats, d_feats, feats.nbytes)
+                    ctx.sync()
+                finally:
+                    ctx.free(d_feats)
             ctx.sync()
-            return split_tiles(self.shapes, inst, table, ro, pred, pts, po)
+            return split_tiles(self.shapes, inst, table, ro, pred, pts, po, feats)
         finally:
             self._free()
 
-    def _rerun(self, rows_cap=None, pts_cap=None):
-        """The group again through the synchronising host variant, with the exact sizes when a capacity check failed."""
+    def _rerun(self, rows_cap=None, pts_cap=None, range_failed=False):
+        """The group again, with the exact sizes when a capacity check failed: through the synchronising host variant,
+        or with features as another TilesJob."""
         self._free()
-        return self.ctx.infer_tiles(self.imgs, self.patch_in, self.batch, want_pred=self.want_pred, contours=self.contours,
-                                    rows_cap=rows_cap, pts_cap=pts_cap)
+        if not self.features:
+            return self.ctx.infer_tiles(self.imgs, self.patch_in, self.batch, want_pred=self.want_pred,
+                                        contours=self.contours, rows_cap=rows_cap, pts_cap=pts_cap)
+        if self.reruns >= self.MAX_RERUNS:
+            raise HvnError(-4 if not range_failed else -6, "tile group with features: reruns exhausted")
+        if range_failed:
+            self.ctx.set_option("act_shift", self.ctx.counter("act_shift") + 6)
+        return TilesJob(self.ctx, self.imgs, self.patch_in, self.batch, self.want_pred, self.contours, True,
+                        rows_cap or self.rows_cap, pts_cap or self.pts_cap, self.reruns + 1).result()
 
 
 class Context:
@@ -516,6 +556,62 @@ class Context:
         check(lib().hvn_valid_loss_dev(self._h, _ptr(d_imgs), _ptr(d_inst), _ptr(d_type), int(B), int(H), int(W),
                                        _ptr(d_counts), _ptr(d_sse), _ptr(d_flags), _ptr(d_sums), _ptr(d_probs)))
 
+    def _features_packed(self, shapes, inst, img, pred, C, table, row_offs, pts, pt_offs):
+        """hvn_inst_features on host arrays already in the packed layout; returns feats [n_rows,FEAT_LEN]."""
+        sh = np.ascontiguousarray(shapes, dtype=np.int32).reshape(-1, 2)
+        n_rows = int(row_offs[-1])
+        feats = np.empty((n_rows, FEAT_LEN), dtype=np.float64)
+        c = lambda a, t: None if a is None else np.ascontiguousarray(a, dtype=t)  # noqa: E731
+        check(lib().hvn_inst_features(
+            self._h, sh.shape[0], _ptr(sh), _ptr(c(inst, np.int32)), _ptr(c(img, np.uint8)), _ptr(c(pred, np.float32)),
+            int(C), _ptr(c(table, np.int64)), _ptr(c(row_offs, np.int32)), n_rows, _ptr(c(pts, np.int32)),
+            _ptr(c(pt_offs, np.int32)), _ptr(feats)))
+        return feats
+
+    def inst_features(self, inst, table, pts, pt_offs, row_offs=None, image=None, pred=None):
+        """Per-instance measurements (hvn_inst_features; columns FEATURE_NAMES) of the rows of `table`.
+        inst: one instance map [H,W] or a list of maps of any sizes; image / pred: None or the matching RGB uint8
+        [H,W,3] (any other dtype is a ValueError) / prediction [H,W,C] maps (NP at channel C - 3; their columns are NaN when None); table [n,10];
+        row_offs [n_maps+1] (default [0, n] for one map); the contour of row r at pts[pt_offs[r]:pt_offs[r+1]], (x, y)
+        in map coordinates.  Returns float64 [n,FEAT_LEN]."""
+        many = isinstance(inst, (list, tuple))
+        maps = [_as_ids(m) for m in (inst if many else [inst])]
+        imgs = None if image is None else [np.asarray(a) for a in (image if many else [image])]
+        if imgs is not None and any(a.dtype != np.uint8 for a in imgs):
+            raise ValueError("images must be uint8 RGB (the colour columns are statistics of 0..255 values), got %s"
+                             % sorted(set(str(a.dtype) for a in imgs)))
+        preds = None if pred is None else [np.asarray(a) for a in (pred if many else [pred])]
+        for k, m in enumerate(maps):
+            if m.ndim != 2 or (imgs is not None and imgs[k].shape != m.shape + (3,)) or \
+                    (preds is not None and (preds[k].ndim != 3 or preds[k].shape[:2] != m.shape)):
+                raise ValueError("map %d: inst [H,W], image [H,W,3] and pred [H,W,C] must agree" % k)
+        C = preds[0].shape[2] if preds is not None else 0
+        table = np.ascontiguousarray(table, dtype=np.int64).reshape(-1, ROW_LEN)
+        if row_offs is None:
+            if many and len(maps) != 1:
+                raise ValueError("row_offs is needed with more than one map")
+            row_offs = [0, table.shape[0]]
+        row_offs = np.ascontiguousarray(row_offs, dtype=np.int32)
+        n_rows = int(row_offs[-1])
+        if n_rows != table.shape[0]:
+            raise ValueError("row_offs[-1] = %d but the table has %d rows" % (n_rows, table.shape[0]))
+        cat = lambda arrs: None if arrs is None else np.concatenate([a.reshape(-1) for a in arrs])  # noqa: E731
+        shapes = np.array([m.shape for m in maps], dtype=np.int32)
+        pts = np.asarray(pts).reshape(-1, 2) if pts is not None else np.zeros((0, 2), np.int32)
+        pt_offs = np.asarray(pt_offs)[: n_rows + 1]
+        if pt_offs.size != n_rows + 1 or not 0 <= int(pt_offs[0]) <= int(pt_offs[-1]) <= pts.shape[0]:
+            raise ValueError("pt_offs needs n_rows + 1 entries with 0 <= pt_offs[0] <= pt_offs[n_rows] <= %d (the "
+                             "points given)" % pts.shape[0])
+        return self._features_packed(shapes, cat(maps), cat(imgs), cat(preds), C, table, row_offs, pts, pt_offs)
+
+    def inst_features_dev(self, n_maps, shapes, d_inst, d_img, d_pred, C, d_table, d_row_offs, n_rows, d_pts, d_pt_offs,
+                          d_feats):
+        """hvn_inst_features_dev on device pointers (shapes: host int32 [n_maps,2]; d_img / d_pred may be None)."""
+        sh = np.ascontiguousarray(shapes, dtype=np.int32)
+        check(lib().hvn_inst_features_dev(self._h, int(n_maps), _ptr(sh), _ptr(d_inst), _ptr(d_img), _ptr(d_pred), int(C),
+                                          _ptr(d_table), _ptr(d_row_offs), int(n_rows), _ptr(d_pts), _ptr(d_pt_offs),
+                                          _ptr(d_feats)))
+
     def mem_get_info(self):
         """(free, total) device bytes of this context's device (hvn_mem_info)."""
         free, total = ctypes.c_size_t(), ctypes.c_size_t()
@@ -559,14 +655,20 @@ class Context:
             return rc, (pred, inst, table[:n], offs, (pts[: int(offs[-1])] if contours else None))
         return _retry_capacity("infer_tile", attempt)
 
-    def infer_tiles(self, imgs, patch_in, batch=0, want_pred=True, contours=True, rows_cap=None, pts_cap=None):
+    def infer_tiles(self, imgs, patch_in, batch=0, want_pred=True, contours=True, rows_cap=None, pts_cap=None,
+                    features=False):
         """A group of RGB images [H_i,W_i,3] of any sizes through the device tile path in one stream of batches
         (hvn_infer_tiles).  Returns one (pred or None, inst, table [k,10], offs or None, pts or None) per image, each
-        equal to infer_tile on that image alone."""
+        equal to infer_tile on that image alone; with features (needs contours) each tuple gains the image's
+        inst_features rows [k,FEAT_LEN], measured on the group's device buffers (a TilesJob) before they are freed."""
+        if features and not contours:
+            raise ValueError("instance features need the contours")
         packed, shapes = pack_images(imgs)
         n = shapes.shape[0]
         if n < 1:
             raise ValueError("infer_tiles needs at least one image")
+        if features:
+            return TilesJob(self, list(imgs), patch_in, batch, want_pred, contours, True, rows_cap, pts_cap).result()
         px = int(packed.size // 3)
         _, _, oc = self.out_shape(patch_in, patch_in)
         r0, p0 = tiles_sizes(shapes)
@@ -595,11 +697,12 @@ class Context:
                 po = po[: rows + 1]
                 pts = pts[: int(po[-1])]
             return rc, (inst, table[:rows], ro, pred, pts, po)
-        return split_tiles(shapes, *_retry_capacity("infer_tiles", attempt))
+        inst, table, ro, pred, pts, po = _retry_capacity("infer_tiles", attempt)
+        return split_tiles(shapes, inst, table, ro, pred, pts, po)
 
-    def infer_tiles_begin(self, imgs, patch_in, batch=0, want_pred=True, contours=True):
+    def infer_tiles_begin(self, imgs, patch_in, batch=0, want_pred=True, contours=True, features=False):
         """Enqueues a tile group with hvn_infer_tiles_dev and returns at once; TilesJob.result() waits for it."""
-        return TilesJob(self, list(imgs), patch_in, batch, want_pred, contours)
+        return TilesJob(self, list(imgs), patch_in, batch, want_pred, contours, features)
 
     def infer_tiles_dev(self, n, d_imgs, shapes, patch_in, batch, d_pred, d_inst, d_table, rows_cap, d_row_offs, d_pts,
                         pts_cap, d_pt_offs):

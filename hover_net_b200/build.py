@@ -9,7 +9,7 @@ LIB = os.path.join(HERE, "libhvn.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
-# (source, extra flags).  postproc.cu must never contract mul+add into FMA (bit-exact float64 stages).
+# (source, extra flags).  postproc.cu and features.cu must never contract mul+add into FMA (bit-exact float64 stages).
 SOURCES = [
     ("api.cu", ["-Xcompiler", "-fvisibility=default"]),
     ("cnn.cu", []),
@@ -22,6 +22,7 @@ SOURCES = [
     ("targets.cu", []),
     ("tta.cu", []),
     ("loss.cu", []),
+    ("features.cu", ["-fmad=false"]),
 ]
 
 

@@ -7,6 +7,7 @@
 
 #include "../../include/hvn.h"
 #include "cnn.h"
+#include "features.h"
 #include "loss.h"
 #include "postproc.h"
 #include "stats.h"
@@ -29,6 +30,7 @@ struct hvn_ctx {
     Arena valid_arena;             // maps and counts of hvn_valid*
     Arena loss_arena;              // per-block partials of hvn_valid_loss*
     Arena group_arena;             // slot table, padded instance tables and slot-order maps of the tile-group path
+    Arena feat_arena;              // map table, status and long-contour scratch of hvn_inst_features*
     void *pin = nullptr;           // pinned staging of the tile-group slot table (uploaded stream-ordered)
     size_t pin_bytes = 0;
     cudaEvent_t pin_ev = nullptr;  // recorded after the last upload from `pin`
@@ -37,7 +39,7 @@ struct hvn_ctx {
     int profile = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t tev[2] = {nullptr, nullptr};
-    float ms_cnn = 0.f, ms_pp = 0.f, ms_loss = 0.f;
+    float ms_cnn = 0.f, ms_pp = 0.f, ms_loss = 0.f, ms_feat = 0.f;
     long long pp_launches = 0;
     std::string pp_log;  // per-kernel post-processing times of the last call ("profile" >= 3)
     std::string log_out;
@@ -165,6 +167,7 @@ void hvn_destroy(hvn_ctx *c) {
     c->valid_arena.release();
     c->loss_arena.release();
     c->group_arena.release();
+    c->feat_arena.release();
     if (c->pin) cudaFreeHost(c->pin);
     if (c->pin_ev) cudaEventDestroy(c->pin_ev);
     for (auto &e : c->ev) cudaEventDestroy(e);
@@ -965,6 +968,102 @@ int hvn_valid_loss(hvn_ctx *c, const uint8_t *imgs, const int32_t *inst, const i
 }
 
 // ---------------------------------------------------------------------------------------------------
+// The map table of a packed feature call; checks the host-side arguments.
+static std::vector<FeatMap> feature_maps(int n, const int32_t *shapes, const float *pred, int C, long long n_rows) {
+    HVN_CHECK(n >= 1 && shapes, HVN_ERR_INVALID, "a feature call needs n_maps >= 1 and their shapes");
+    HVN_CHECK(!pred || C >= 3, HVN_ERR_INVALID, "a prediction map needs C >= 3 channels (NP at C - 3)");
+    HVN_CHECK(n_rows >= 0 && n_rows < (1ll << 31) - 1, HVN_ERR_INVALID, "n_rows must be in 0 .. 2^31 - 2");
+    std::vector<FeatMap> maps(n);
+    long long off = 0;
+    for (int m = 0; m < n; ++m) {
+        const int H = shapes[2 * m], W = shapes[2 * m + 1];
+        HVN_CHECK(H >= 1 && W >= 1 && (long long)H * W < (1ll << 31), HVN_ERR_INVALID,
+                  "map " + std::to_string(m) + ": bad shape " + std::to_string(H) + "x" + std::to_string(W));
+        maps[m] = {off, H, W};
+        off += (long long)H * W;
+    }
+    return maps;
+}
+
+// hvn_inst_features_dev on device buffers: the check, one synchronisation to read its status, then the measurements.
+static void run_features(hvn_ctx *c, const std::vector<FeatMap> &maps, const int32_t *inst, const uint8_t *img,
+                         const float *pred, int C, const int64_t *table, const int32_t *row_offs, long long n_rows,
+                         const int32_t *pts, const int32_t *pt_offs, double *feats) {
+    HVN_CHECK(inst && table && row_offs && pt_offs && (feats || n_rows == 0), HVN_ERR_INVALID, "null buffer");
+    const int n = (int)maps.size();
+    FeatMap *d_maps;
+    FeatStatus *d_st, st;
+    void *scratch = nullptr;
+    size_t scratch_bytes = 0;
+    auto layout = [&](Buffers &b) {
+        d_maps = b.in(maps.data(), maps.size());
+        d_st = b.scratch<FeatStatus>(1);
+        scratch = scratch_bytes ? b.scratch<char>(scratch_bytes) : nullptr;
+    };
+    Buffers ws(c, c->feat_arena, layout);
+    if (c->profile) HVN_CUDA(cudaEventRecord(c->ev[2], c->stream));
+    c->pp_launches += features_check(c->stream, d_maps, n, row_offs, n_rows, (const long long *)table, pts, pt_offs, d_st);
+    HVN_CUDA(cudaMemcpyAsync(&st, d_st, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+    HVN_CUDA(cudaStreamSynchronize(c->stream));
+    HVN_CHECK(!(st.err & 1), HVN_ERR_INVALID, "row_offs must rise from 0 to n_rows = " + std::to_string(n_rows));
+    HVN_CHECK(!(st.err & 2), HVN_ERR_INVALID, "a table row's bbox is empty or outside its map");
+    HVN_CHECK(!(st.err & 4), HVN_ERR_INVALID, "pt_offs must not fall (and pt_offs[0] >= 0)");
+    HVN_CHECK(!(st.err & 8), HVN_ERR_INVALID, "a contour point lies outside its row's bbox");
+    if (st.max_pts > FEAT_SMEM_POINTS) {  // long contours: the arena again, now with their scratch (the stream is idle)
+        scratch_bytes = FEAT_SCRATCH_BYTES_PER_POINT * (size_t)st.total_pts;
+        Buffers again(c, c->feat_arena, layout);
+    }
+    c->pp_launches += features_rows(c->stream, d_maps, n, inst, img, pred, C, (const long long *)table, row_offs, n_rows,
+                                    pts, pt_offs, scratch, feats, st.total_pts);
+    if (c->profile) {
+        HVN_CUDA(cudaEventRecord(c->ev[3], c->stream));
+        HVN_CUDA(cudaStreamSynchronize(c->stream));
+        HVN_CUDA(cudaEventElapsedTime(&c->ms_feat, c->ev[2], c->ev[3]));
+    }
+}
+
+int hvn_inst_features_dev(hvn_ctx *c, int n, const int32_t *shapes, const int32_t *inst, const uint8_t *img,
+                          const float *pred, int C, const int64_t *table, const int32_t *row_offs, int64_t n_rows,
+                          const int32_t *pts, const int32_t *pt_offs, double *feats) {
+    API_BEGIN
+    use(c);
+    run_features(c, feature_maps(n, shapes, pred, C, n_rows), inst, img, pred, C, table, row_offs, n_rows, pts, pt_offs,
+                 feats);
+    API_END
+}
+
+int hvn_inst_features(hvn_ctx *c, int n, const int32_t *shapes, const int32_t *inst, const uint8_t *img,
+                      const float *pred, int C, const int64_t *table, const int32_t *row_offs, int64_t n_rows,
+                      const int32_t *pts, const int32_t *pt_offs, double *feats) {
+    API_BEGIN
+    use(c);
+    const std::vector<FeatMap> maps = feature_maps(n, shapes, pred, C, n_rows);
+    HVN_CHECK(inst && table && row_offs && pt_offs && (feats || n_rows == 0), HVN_ERR_INVALID, "null buffer");
+    // the points the offsets reach are staged; the device check sees the offsets themselves
+    HVN_CHECK(pt_offs[0] >= 0 && pt_offs[n_rows] >= pt_offs[0] && (pts || pt_offs[n_rows] == 0), HVN_ERR_INVALID,
+              "pt_offs must not fall (and pt_offs[0] >= 0)");
+    const size_t px = (size_t)(maps.back().px_off + (long long)maps.back().H * maps.back().W);
+    const uint8_t *d_img;
+    const float *d_pred;
+    const int32_t *d_inst, *d_ro, *d_pts, *d_po;
+    const int64_t *d_tab;
+    double *d_feats;
+    Buffers io(c, c->io_arena, [&](Buffers &s) {
+        d_inst = s.in(inst, px);
+        d_img = img ? s.in(img, px * 3) : nullptr;
+        d_pred = pred ? s.in(pred, px * C) : nullptr;
+        d_tab = s.in(table, (size_t)n_rows * HVN_ROW_LEN);
+        d_ro = s.in(row_offs, (size_t)n + 1);
+        d_pts = s.in(pts, (size_t)pt_offs[n_rows] * 2);
+        d_po = s.in(pt_offs, (size_t)n_rows + 1);
+        d_feats = s.out(feats, (size_t)n_rows * HVN_FEAT_LEN);
+    });
+    run_features(c, maps, d_inst, d_img, d_pred, C, d_tab, d_ro, n_rows, d_pts, d_po, d_feats);
+    io.copy_back();
+    API_END
+}
+
+// ---------------------------------------------------------------------------------------------------
 int hvn_malloc(hvn_ctx *c, size_t bytes, void **p) {
     API_BEGIN
     use(c);
@@ -1054,6 +1153,7 @@ int hvn_stage_ms(const hvn_ctx *c, const char *name, float *ms) {
     if (k == "cnn") *ms = c->ms_cnn;
     else if (k == "postproc") *ms = c->ms_pp;
     else if (k == "loss") *ms = c->ms_loss;
+    else if (k == "features") *ms = c->ms_feat;
     else if (c->model && c->model->class_ms.count(k)) *ms = (float)c->model->class_ms.at(k);
     else if (k == "conv_tc" || k == "conv_ref" || k == "conv0" || k == "bnrelu" || k == "head" || k == "tta") *ms = 0.f;
     else throw Error(HVN_ERR_INVALID, "unknown stage " + k);

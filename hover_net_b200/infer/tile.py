@@ -8,7 +8,12 @@ reference's RAM budget (`mem_usage` of the available RAM, `sys.getsizeof(padded 
 by half of the free device memory; the patches of a whole group run as one stream of `batch_size` batches that span
 image boundaries (`hvn_infer_tiles`), and equal-size images are post-processed together.  On one GPU a group runs on
 the device while the previous group's files are written and the next group's files are read.  Unlike the reference, a
-file that exceeds the budget on its own is processed as a group of one instead of being skipped."""
+file that exceeds the budget on its own is processed as a group of one instead of being skipped.
+
+Extension the reference lacks: run arg `save_features` (`run_infer.py tile --save_features`) measures every nucleus on the
+device (`_lib.FEATURE_NAMES`: shape, colour and NP-probability statistics, hvn_inst_features) before the group's device
+maps are freed.  The JSON records gain "features" and the `.mat` gains `inst_features` [n,18] (rows in `inst_uid`
+order) and `inst_feature_names`."""
 import glob
 import math
 import os
@@ -131,6 +136,9 @@ def _to_qupath(file_path, nuc_pos_list, nuc_type_list, type_info_dict):
 # its slot entry.
 DEVICE_BYTES_PER_PX = 192
 DEVICE_BYTES_PER_FILE = 40 << 10
+# With save_features: the prediction map the group keeps on the device for np_prob_mean (16) and the feature rows
+# (18 x 8 B per table row, at most one row per 64 px by default: ~2.3).
+FEATURE_BYTES_PER_PX = 20
 _END = object()
 
 
@@ -141,11 +149,13 @@ def _padded_shape(h, w, win, step):
     return last(h) + win + padt, last(w) + win + padt, 3
 
 
-def _file_cost(shape, win, step):
+def _file_cost(shape, win, step, features=False):
     """(RAM, device) bytes charged for one image of shape [H,W,3]: the reference's `sys.getsizeof(padded image) * 5`
-    (infer/tile.py:271) and DEVICE_BYTES_PER_PX per pixel plus DEVICE_BYTES_PER_FILE."""
+    (infer/tile.py:271) and DEVICE_BYTES_PER_PX (+ FEATURE_BYTES_PER_PX with features) per pixel plus
+    DEVICE_BYTES_PER_FILE."""
     ram = sys.getsizeof(np.empty(_padded_shape(shape[0], shape[1], win, step), dtype=np.uint8)) * 5
-    return ram, DEVICE_BYTES_PER_PX * int(shape[0]) * int(shape[1]) + DEVICE_BYTES_PER_FILE
+    per_px = DEVICE_BYTES_PER_PX + (FEATURE_BYTES_PER_PX if features else 0)
+    return ram, per_px * int(shape[0]) * int(shape[1]) + DEVICE_BYTES_PER_FILE
 
 
 def _groups(items, costs, budgets):
@@ -195,9 +205,12 @@ class InferManager(base.InferManager):
 
         dist, rank, world = dist_info()
         win = int(self.patch_input_shape)
+        feats = getattr(self, "save_features", False)
         if getattr(self, "device_tile_path", False) and (world == 1 or dist.get_backend() == "nccl"):
             ctx = self.net.ctx
             if world == 1:
+                if feats:
+                    return self.infer_images([img])[0]
                 pred_map, pred_inst, table, offs, pts = ctx.infer_tile(img, win, self.batch_size)
                 return np.squeeze(pred_map), pred_inst, table_to_dict(table, offs, pts, self.nr_types)
             import torch
@@ -216,13 +229,17 @@ class InferManager(base.InferManager):
                 if rank != 0:
                     return None, None, None
             # whole-map post-processing + contours on the reduced map where it already lives: no 268 MB host round trip
-            pred_inst, inst_info_dict = self._post_process_on_device(ctx, d_pred, H, W)
+            pred_inst, inst_info_dict = self._post_process_on_device(ctx, d_pred, H, W, d_img if feats else None)
             return np.squeeze(d_pred.cpu().numpy()), pred_inst, inst_info_dict
         else:
             src_shape = img.shape
             padded, patch_info, _ = _prepare_patching(img, self.patch_input_shape, self.patch_output_shape, True)
             outs = run_patches(padded, patch_info, self.patch_input_shape, self.run_step, self.batch_size)
             pred_map = _stitch(patch_info, outs, src_shape)
+        if feats:
+            from ..models.hovernet.post_proc import process_features
+            pred_inst, inst_info_dict = process_features(pred_map, nr_types=self.nr_types, image=img)
+            return np.squeeze(pred_map), pred_inst, inst_info_dict
         pred_inst, inst_info_dict = self.post_proc_func(pred_map, nr_types=self.nr_types, return_centroids=True)
         return np.squeeze(pred_map), pred_inst, inst_info_dict
 
@@ -243,9 +260,10 @@ class InferManager(base.InferManager):
         if not (getattr(self, "device_tile_path", False) and (world == 1 or dist.get_backend() == "nccl")):
             return [self.infer_image(img, all_ranks=all_ranks) for img in imgs]
         ctx = self.net.ctx
+        feats = getattr(self, "save_features", False)
         if world == 1:
-            return [(np.squeeze(p), i, table_to_dict(t, o, pts, self.nr_types))
-                    for p, i, t, o, pts in ctx.infer_tiles(imgs, win, self.batch_size)]
+            return [(np.squeeze(r[0]), r[1], table_to_dict(r[2], r[3], r[4], self.nr_types, r[5] if feats else None))
+                    for r in ctx.infer_tiles(imgs, win, self.batch_size, features=feats)]
         import torch
         C = ctx.out_shape(win, win)[2]
         grids = [ctx.tile_grid(img.shape[0], img.shape[1], win) for img in imgs]
@@ -272,14 +290,18 @@ class InferManager(base.InferManager):
         for i, img in enumerate(imgs):
             H, W = img.shape[:2]
             m = d_pred[int(px[i]) * C:int(px[i + 1]) * C].view(H, W, C)
-            pred_inst, inst_info_dict = self._post_process_on_device(ctx, m, H, W)
+            d_img = None
+            if feats:
+                d_img = d_imgs[i] if i in d_imgs else torch.from_numpy(np.ascontiguousarray(img)).cuda()
+            pred_inst, inst_info_dict = self._post_process_on_device(ctx, m, H, W, d_img)
             out.append((np.squeeze(m.cpu().numpy()), pred_inst, inst_info_dict))
         return out
 
-    def _post_process_on_device(self, ctx, d_pred, H, W):
+    def _post_process_on_device(self, ctx, d_pred, H, W, d_img=None):
         """`process` (post_proc.py:94-186) on a device-resident map [H,W,C]: hvn_postproc_dev + hvn_contours_dev, then
         only the instance map, the table rows and the contour points come back.  Same kernels as `post_proc.process`,
-        hence the same result."""
+        hence the same result.  With d_img (the image [H,W,3] u8 on the device) the instances are also measured there
+        (hvn_inst_features_dev)."""
         import torch
         from ..models.hovernet.post_proc import table_to_dict
         C = int(d_pred.shape[-1])
@@ -305,7 +327,18 @@ class InferManager(base.InferManager):
                 cap = total
                 continue
             table = d_tab[:n].cpu().numpy()
-            info = table_to_dict(table, d_offs.cpu().numpy(), d_pts[:total].cpu().numpy(), self.nr_types)
+            feats = None
+            if d_img is not None:
+                from .. import _lib
+                d_ro = torch.tensor([0, n], dtype=torch.int32, device=d_pred.device)
+                d_feats = torch.empty((max(1, n), _lib.FEAT_LEN), dtype=torch.float64, device=d_pred.device)
+                torch.cuda.synchronize()
+                ctx.inst_features_dev(1, [[H, W]], d_inst.data_ptr(), d_img.data_ptr(), d_pred.data_ptr(), C,
+                                      d_tab.data_ptr(), d_ro.data_ptr(), n, d_pts.data_ptr(), d_offs.data_ptr(),
+                                      d_feats.data_ptr())
+                ctx.sync()
+                feats = d_feats[:n].cpu().numpy()
+            info = table_to_dict(table, d_offs.cpu().numpy(), d_pts[:total].cpu().numpy(), self.nr_types, feats)
             return d_inst.cpu().numpy(), info
         raise RuntimeError("tile post-processing: capacity retries exhausted")
 
@@ -317,6 +350,7 @@ class InferManager(base.InferManager):
 
         self.save_qupath = False
         self.save_raw_map = False
+        self.save_features = False
         self.draw_dot = False
         self.mem_usage = 0.1
         self.batch_size = 32
@@ -357,7 +391,8 @@ class InferManager(base.InferManager):
             # tail builds one, up to ~18 GB for 32 original-mode patches) and the patch batches
             return ram, (ctx.mem_get_info()[0] // 2 if ctx is not None else None)
 
-        groups = _groups((read(p) for p in file_path_list), lambda f: _file_cost(f[1].shape, win, step), budgets)
+        groups = _groups((read(p) for p in file_path_list),
+                         lambda f: _file_cost(f[1].shape, win, step, self.save_features), budgets)
         if not overlap:
             for files in groups:
                 results = self.infer_images([img for _, img in files])
@@ -369,12 +404,14 @@ class InferManager(base.InferManager):
         files = next(groups, None)
         done = None  # (files, results) of the group whose outputs are still to be written
         while files is not None:
-            job = ctx.infer_tiles_begin([img for _, img in files], win, self.batch_size, want_pred=self.save_raw_map)
+            job = ctx.infer_tiles_begin([img for _, img in files], win, self.batch_size, want_pred=self.save_raw_map,
+                                        features=self.save_features)
             if done is not None:
                 self._write_files(*done)
             upcoming = next(groups, None)
-            results = [(None if p is None else np.squeeze(p), i, table_to_dict(t, o, pts, self.nr_types))
-                       for p, i, t, o, pts in job.result()]
+            results = [(None if r[0] is None else np.squeeze(r[0]), r[1],
+                        table_to_dict(r[2], r[3], r[4], self.nr_types, r[5] if self.save_features else None))
+                       for r in job.result()]
             done = (files, results)
             files = upcoming
         if done is not None:
@@ -383,9 +420,11 @@ class InferManager(base.InferManager):
 
     def _write_files(self, files, results):
         """The outputs of one group, file after file: `.mat`, overlay, QuPath TSV and JSON (reference
-        infer/tile.py:326-369)."""
+        infer/tile.py:326-369); with `save_features` also the `.mat`'s feature table."""
         import cv2
         import scipy.io as sio
+
+        from .. import _lib
 
         for (file_path, img), (pred_map, pred_inst, inst_info_dict) in zip(files, results):
             img_name = pathlib.Path(file_path).stem
@@ -399,6 +438,10 @@ class InferManager(base.InferManager):
                 mat_dict.pop("inst_type", None)
             if self.save_raw_map:
                 mat_dict["raw_map"] = pred_map
+            if getattr(self, "save_features", False):
+                mat_dict["inst_features"] = np.array([[v["features"].get(k, np.nan) for k in _lib.FEATURE_NAMES]
+                                                      for v in nuc_val_list], dtype=np.float64).reshape(-1, _lib.FEAT_LEN)
+                mat_dict["inst_feature_names"] = np.array(_lib.FEATURE_NAMES, dtype=object)
             sio.savemat("%s/mat/%s.mat" % (self.output_dir, img_name), mat_dict)
 
             overlaid = _overlay(img, inst_info_dict, draw_dot=self.draw_dot,

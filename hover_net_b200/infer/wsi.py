@@ -16,6 +16,13 @@ What changes underneath:
   reference produces with `nr_post_proc_workers=0` (with a pool its order is completion order).
 * slides: `.npy` arrays and ordinary image files are read natively; OpenSlide formats need the
   `openslide` module (absent from this image) and raise a clear error otherwise.
+
+Extension the reference lacks: run arg `save_features` (`run_infer.py wsi --save_features`) measures every nucleus of
+every post-processing tile on the device (`_lib.FEATURE_NAMES`) on the tile's instance map, its region of the slide and
+its prediction map, so each record carries "features" through the merge.  A nucleus cut by a tile edge is measured on
+the same truncated pixels as its contour and bbox.  The merge never changes the pixels of a nucleus it keeps (a kept
+old nucleus is left as it is, a new one is added only where it overlaps no kept one), so every written record's
+features are those of its pixels in the final instance map.
 """
 import glob
 import logging
@@ -261,13 +268,21 @@ class InferManager(base.InferManager):
         """Post-process every tile (sharded over the ranks) and feed the results to `callback` in tile
         order on rank 0 (reference wsi.py:385-437 with nr_post_proc_workers=0)."""
         dist, rank, world = _dist_info()
-        kwargs = {"nr_types": self.method["model_args"]["nr_types"], "return_centroids": True}
+        nr_types = self.method["model_args"]["nr_types"]
+        features = getattr(self, "save_features", False)
+        if features:
+            from ..models.hovernet.post_proc import process_features
         n = tile_info_list.shape[0]
         mine = []
         for idx in range(rank, n, world):
             tl, br = tile_info_list[idx][0], tile_info_list[idx][1]
             tile_pred = np.array(self.wsi_pred_map[tl[0] : br[0], tl[1] : br[1]])
-            mine.append((self.post_proc_func(tile_pred, **kwargs), (idx, tl, br)))
+            if features:  # with the tile's region of the slide, at the processing magnification
+                region = np.ascontiguousarray(self.wsi_handler.read_region(tl[::-1], (br - tl)[::-1]))
+                res = process_features(tile_pred, nr_types=nr_types, image=region)
+            else:
+                res = self.post_proc_func(tile_pred, nr_types=nr_types, return_centroids=True)
+            mine.append((res, (idx, tl, br)))
         if world > 1:
             gathered = [None] * world if rank == 0 else None
             dist.gather_object(mine, gathered, dst=0)
@@ -424,6 +439,7 @@ class InferManager(base.InferManager):
         """Every slide under run_args['input_dir'] (reference wsi.py:711-753)."""
         self.save_thumb = False
         self.save_mask = False
+        self.save_features = False
         self.input_mask_dir = None
         self.cache_path = "cache"
         self._parse_args(run_args)

@@ -20,6 +20,12 @@ Extension the reference CLI lacks: `--tta` (test-time augmentation) runs every p
 (4 rotations x optional mirror) and averages their maps on the device, the HV vectors mapped back to the patch's
 frame, before post-processing: eight times the network work.  When given, `"tta": True` is added to `model_args`;
 tile and WSI modes take it from the model.
+
+Extension the reference CLI lacks: `--save_features` (tile and wsi) measures every nucleus on the device -- area,
+contour and convex areas, perimeter, solidity, circularity, ellipse axes, eccentricity, orientation, maximum Feret
+diameter, mean and standard deviation of each RGB channel, and the mean NP probability -- and adds them to each JSON
+record as "features" (tile mode also to the `.mat` as `inst_features` / `inst_feature_names`).  Without it every output
+is what the reference writes.
 """
 import argparse
 import logging
@@ -53,6 +59,7 @@ def _tile_parser():
     ap.add_argument("--draw_dot", action="store_true")
     ap.add_argument("--save_qupath", action="store_true")
     ap.add_argument("--save_raw_map", action="store_true")
+    ap.add_argument("--save_features", action="store_true")
     return ap
 
 
@@ -68,6 +75,7 @@ def _wsi_parser():
     ap.add_argument("--tile_shape", default="2048")
     ap.add_argument("--save_thumb", action="store_true")
     ap.add_argument("--save_mask", action="store_true")
+    ap.add_argument("--save_features", action="store_true")
     return ap
 
 
@@ -117,6 +125,8 @@ def parse(argv, nr_gpus=1):
             "chunk_shape": int(sub.chunk_shape), "tile_shape": int(sub.tile_shape),
             "save_thumb": sub.save_thumb, "save_mask": sub.save_mask,
         })
+    if sub.save_features:  # the default leaves run_args exactly as the reference builds them
+        run_args["save_features"] = True
     return sub_cmd, method_args, run_args, args.gpu
 
 

@@ -49,6 +49,13 @@ typedef enum {
 enum { HVN_ROW_ID = 0, HVN_ROW_RMIN, HVN_ROW_CMIN, HVN_ROW_RMAX, HVN_ROW_CMAX, HVN_ROW_AREA,
        HVN_ROW_SUMX, HVN_ROW_SUMY, HVN_ROW_TYPE, HVN_ROW_TYPECNT };
 
+/* Per-instance measurements (hvn_inst_features*): HVN_FEAT_LEN float64 per instance-table row, in this order. */
+#define HVN_FEAT_LEN 18
+enum { HVN_FEAT_AREA = 0, HVN_FEAT_CONTOUR_AREA, HVN_FEAT_PERIMETER, HVN_FEAT_CONVEX_AREA, HVN_FEAT_SOLIDITY,
+       HVN_FEAT_CIRCULARITY, HVN_FEAT_MAJOR_AXIS_LENGTH, HVN_FEAT_MINOR_AXIS_LENGTH, HVN_FEAT_ECCENTRICITY,
+       HVN_FEAT_ORIENTATION, HVN_FEAT_FERET_MAX, HVN_FEAT_MEAN_R, HVN_FEAT_MEAN_G, HVN_FEAT_MEAN_B, HVN_FEAT_STD_R,
+       HVN_FEAT_STD_G, HVN_FEAT_STD_B, HVN_FEAT_NP_PROB_MEAN };
+
 typedef struct hvn_ctx hvn_ctx;
 
 int hvn_abi_version(void);
@@ -101,9 +108,9 @@ int hvn_finalize_weights(hvn_ctx *ctx);
  *                      fp32-accumulation noise (tests/test_cnn_gpu.py::test_kernel_variants_agree). */
 int hvn_set_option(hvn_ctx *ctx, const char *key, int64_t value);
 const char *hvn_debug_log(const hvn_ctx *ctx);
-/* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing and contour kernels), "tile_table_rows" (rows
- * of padded instance tables the last hvn_infer_tiles* group of two or more images held in the context's workspace:
- * min(rows_cap, H*W/6 + 8) per image, 84 B each), "last_flops" (algorithmic 2*MACs of the
+/* counters: "kernel_launches", "tc_launches", "pp_launches" (post-processing, contour and feature kernels),
+ * "tile_table_rows" (rows of padded instance tables the last hvn_infer_tiles* group of two or more images held in the
+ * context's workspace: min(rows_cap, H*W/6 + 8) per image, 84 B each), "last_flops" (algorithmic 2*MACs of the
  * last forward; with "tta" = 1 the 8 views' work), "precision" (0 | 1), "tta" (0 | 1), "plan_bytes" (device bytes of
  * the activation buffers, and with "tta" = 1 the per-chunk view and probability workspace, of the plan(s) the last
  * forward ran); with option "profile" = 2 also "launches:<class>" and "flops:<class>" for
@@ -268,6 +275,39 @@ int hvn_valid_loss_dev(hvn_ctx *ctx, const uint8_t *imgs_dev, const int32_t *ins
                        int H, int W, int64_t *counts_dev, double *hv_sse_dev, int32_t *flags_dev, double *sums_dev,
                        float *probs_dev);
 
+/* ---- per-instance measurements (an extension; the reference has no such output): for every instance-table row, the
+ * HVN_FEAT_LEN columns below, in float64.  Layout of hvn_infer_tiles: n_maps >= 1 maps of any sizes back to back,
+ * shapes [n_maps][2] = (H, W) a host array in both variants; inst int32 [H_i,W_i]; img u8 [H_i,W_i,3] RGB or NULL;
+ * pred float32 [H_i,W_i,C] or NULL, its NP probability at channel C - 3 (C >= 3); table [n_rows,10] with the rows of
+ * map m at [row_offs[m], row_offs[m+1]); the contour of row r at pts[pt_offs[r] : pt_offs[r+1]] ((x, y) int32 in map
+ * coordinates, as hvn_contours / hvn_infer_tiles write it; pts holds pt_offs[n_rows] points, the host variant stages
+ * that many); feats [n_rows,HVN_FEAT_LEN].  n_rows is a host argument
+ * equal to row_offs[n_maps] (0 is allowed: nothing is written).  A one-map hvn_postproc_contours result is this layout
+ * with row_offs = {0, n}, pt_offs = offs.  With A the pixels of inst == id in the row's bbox, x, y relative to
+ * (cmin, rmin), P the row's points:
+ *   AREA A;  CONTOUR_AREA cv2.contourArea(P);  PERIMETER cv2.arcLength(P, closed) (fp32 segment lengths, fp64 sum in
+ *   point order from the closing segment);  CONVEX_AREA cv2.contourArea(cv2.convexHull(P));  SOLIDITY contour_area /
+ *   convex_area;  CIRCULARITY 4 pi contour_area / perimeter^2;  MAJOR/MINOR_AXIS_LENGTH 4 sqrt(l1), 4 sqrt(l2),
+ *   ECCENTRICITY sqrt(1 - l2 / l1), ORIENTATION 0.5 atan2(2b, a - c) (radians from the x axis, y down), with a, b, c
+ *   = mu20, mu11, mu02 of cv2.moments(crop == id, binaryImage) over A, r = sqrt(((a - c) / 2)^2 + b^2), l1 =
+ *   (a + c) / 2 + r, l2 = max((a + c) / 2 - r, 0);  FERET_MAX the largest distance between two points of P;
+ *   MEAN_R/G/B S_c / A and STD_R/G/B sqrt((A Q_c - S_c^2) / A^2) (population std; S_c, Q_c the exact sums of the
+ *   channel and of its squares, the numerator exact and rounded once);  NP_PROB_MEAN the fp64 mean of the NP values.
+ * A zero denominator gives 0.0; columns 11-16 are NaN without img, column 17 NaN without pred.  Columns 0-16 are
+ * bit-exact (ORIENTATION within 4 ulp); NP_PROB_MEAN's sum has a fixed order, so repeated calls are bit-identical.
+ * HVN_ERR_INVALID on a bad shape, C < 3 with pred, row_offs not rising from 0 to n_rows, falling pt_offs, a bbox
+ * outside its map or empty, or a point outside its row's bbox.  Device workspace (context-owned, grow-only): 16 B per
+ * map, and 24 B per contour point of the call when a row has more than 512 points (rows up to 512 points are hulled in
+ * shared memory).  Both variants synchronise the context stream once, after the argument check, to report the status;
+ * the _dev variant's measurements are then stream-ordered on the context stream (hvn_sync waits for them).  Option
+ * "profile" = 1 reports the call's device time as stage "features"; the kernels count towards "pp_launches". */
+int hvn_inst_features(hvn_ctx *ctx, int n_maps, const int32_t *shapes, const int32_t *inst_host, const uint8_t *img_host,
+                      const float *pred_host, int C, const int64_t *table_host, const int32_t *row_offs_host,
+                      int64_t n_rows, const int32_t *pts_host, const int32_t *pt_offs_host, double *feats_host);
+int hvn_inst_features_dev(hvn_ctx *ctx, int n_maps, const int32_t *shapes, const int32_t *inst_dev, const uint8_t *img_dev,
+                          const float *pred_dev, int C, const int64_t *table_dev, const int32_t *row_offs_dev,
+                          int64_t n_rows, const int32_t *pts_dev, const int32_t *pt_offs_dev, double *feats_dev);
+
 /* ---- device memory / stream helpers for callers without a CUDA binding of their own. */
 int hvn_malloc(hvn_ctx *ctx, size_t bytes, void **dev_ptr);
 int hvn_free(hvn_ctx *ctx, void *dev_ptr);
@@ -283,8 +323,8 @@ int hvn_mem_info(hvn_ctx *ctx, size_t *free_bytes, size_t *total_bytes);
 int hvn_timer_start(hvn_ctx *ctx);
 int hvn_timer_stop(hvn_ctx *ctx, float *ms);
 /* device time (ms) of the last forward / postproc call.  option "profile" = 1: name in
- * {"cnn","postproc","loss"} (whole stage, CUDA events on the context stream; "loss": the reduction of the last
- * hvn_valid_loss* call).  "profile" = 2 additionally
+ * {"cnn","postproc","loss","features"} (whole stage, CUDA events on the context stream; "loss": the reduction of the
+ * last hvn_valid_loss* call; "features": the last hvn_inst_features* call).  "profile" = 2 additionally
  * brackets every CNN launch with its own event pair and sums per kernel class:
  * {"conv_tc","conv_ref","conv0","bnrelu","head","tta"} ("tta": the view and merge kernels of option "tta"). */
 int hvn_stage_ms(const hvn_ctx *ctx, const char *name, float *ms);
