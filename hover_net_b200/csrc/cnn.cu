@@ -426,7 +426,9 @@ void Model::selftest_conv(const Op &op, cudaStream_t s) {
     unsigned int *d_out = (unsigned int *)dz(16);
     const bool trace = getenv("HVN_TRACE") != nullptr;
     if (trace) { fprintf(stderr, "[selftest] %s ...\n", op.name.c_str()); fflush(stderr); }
-    tc_launch(a, op.tc, s);
+    TcPlan pa;   // the plan's tensor maps address the epilogue tensors: planned again for the scratch outputs
+    HVN_CHECK(tc_plan(a, pa), -1, "selftest: tc_plan declined the scratch outputs of a planned layer");
+    tc_launch(a, pa, s);
     if (b.in_scale) {  // referee path of a transformed-input layer: BN+ReLU pass into the scratch view, then the conv
         launch_bnrelu(b.a_raw, B, b.in_scale, b.in_shift, b.a, s);
         b.in_scale = b.in_shift = nullptr;
@@ -858,11 +860,22 @@ void Model::forward(const uint8_t *imgs, int B, int H, int W, float *out, int ch
             if (profile_ops >= 2) {
                 char line[384];
                 const Op *o = r.op;
-                if (o && o->kind == Op::CONV)
-                    snprintf(line, sizeof(line), "%-44s %-8s k%dx%d s%d cin%-4d cout%-4d out%dx%d box=%dx%d bn=%d %8.4f ms %8.2f GFLOP %7.1f TFLOP/s\n",
+                if (o && o->kind == Op::CONV) {
+                    // algorithmic HBM bytes: every input read once, every output written once, weights ignored
+                    const ConvParams &c = o->cp;
+                    const double px = (double)c.B * c.ho * c.wo, up = c.up2 ? 4.0 : 1.0;
+                    auto split_b = [](const SplitRef &v) { return v.lo ? 4.0 : 2.0; };
+                    double by = c.in_scale ? (double)c.B * c.a_raw.h * c.a_raw.w * c.a_raw.c * 4.0
+                                           : (double)c.B * c.a.h * c.a.w * c.a.c * split_b(c.a);
+                    if (c.a2.hi) by += (double)c.B * c.a2.h * c.a2.w * c.a2.c * split_b(c.a2);
+                    if (c.res.p) by += px * c.w.cout * 4.0;
+                    if (c.out_raw.p) by += px * c.w.cout * 4.0;
+                    if (c.out_split.hi) by += up * px * c.w.cout * split_b(c.out_split);
+                    if (c.up2) by += up * px * c.w.cout * split_b(c.skip);
+                    snprintf(line, sizeof(line), "%-44s %-8s k%dx%d s%d cin%-4d cout%-4d out%dx%d box=%dx%d bn=%d %8.4f ms %8.2f GFLOP %7.1f TFLOP/s %8.4f GB\n",
                              o->name.c_str(), r.cls, o->cp.w.kh, o->cp.w.kw, o->cp.stride, o->cp.w.cin, o->cp.w.cout, o->cp.ho, o->cp.wo,
-                             o->tc.bw, o->tc.bh, o->tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f));
-                else
+                             o->tc.bw, o->tc.bh, o->tc.block_n, ms, r.flops / 1e9, r.flops / 1e9 / std::max(ms, 1e-6f), by / 1e9);
+                } else
                     snprintf(line, sizeof(line), "%-44s %-8s %8.4f ms\n", o ? o->name.c_str() : r.name, r.cls, ms);
                 debug_log += line;
             }

@@ -45,6 +45,10 @@ struct TcPlan {
     bool ok = false;
     unsigned char tmap_a_hi[128], tmap_a_lo[128], tmap_w_hi[128], tmap_w_lo[128];
     unsigned char tmap_a2_hi[128], tmap_a2_lo[128];  // second GEMM source (fused shortcut), if any
+    // epilogue tensors, 32-channel boxes of one M-tile: residual (load), raw and split outputs (bulk stores)
+    unsigned char tmap_res[128], tmap_out_raw[128], tmap_out_hi[128], tmap_out_lo[128];
+    int epi_tma = 0;             // 1: the epilogue tensors move by TMA; 0: a flat tile over a cropped view, copied by
+                                 // the consumer threads from the same shared-memory staging (no TMA box describes it)
     int bw = 0, bh = 0;          // M-tile = bw x bh output pixels of one image
     int tiles_x = 0, tiles_y = 0;
     int block_n = 0;

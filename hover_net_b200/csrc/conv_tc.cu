@@ -16,8 +16,10 @@
 //   operand precision of TF32.  The freed shared memory holds more stages; the epilogue stores hi only.
 // * Persistent CTAs (one per SM), warp-specialised: warp 0 = TMA producer; warpgroups 1 and 2 = consumers, each issuing
 //   the wgmma of 64 of the tile's 128 pixel rows over all BLOCK_N columns and running the fused epilogue (BN/ReLU/
-//   residual/upsample -> global) straight from its accumulator fragment.  A shared-memory ring of STAGES operand slots
-//   lets the producer run ahead, also across the consumers' epilogue.
+//   residual/upsample) from its accumulator fragment.  A shared-memory ring of STAGES operand slots lets the producer
+//   run ahead, also across the consumers' epilogue.
+// * Epilogue tensors move by TMA (plain and residual epilogues): the producer loads the residual into a staging ring,
+//   the consumers finish each 32-channel chunk there and one thread stores it with bulk tensor stores.
 // * Accumulation precision: the K loop is cut into segments of G.seg 64-channel slices; each segment accumulates in the
 //   wgmma registers from zero and is then added into a separate fp32 sum with round-to-nearest adds, so the number of
 //   products chained inside the tensor core stays bounded however large K is.
@@ -75,6 +77,22 @@ __device__ __forceinline__ void tma_4d(uint32_t dst, const void *tmap, uint32_t 
     asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
                  ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+// Bulk tensor stores shared -> global (epilogue).  Elements outside the tensor map's extent are not written.
+__device__ __forceinline__ void tma_store_2d(const void *tmap, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(tmap), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const void *tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(tmap), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still reading shared memory / still writing global memory
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// the 256 consumer threads (warpgroups 1, 2)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
 // L2 prefetch of a tensor-map box: no shared memory, no barrier -- used to run several K-slices ahead of the loads on
 // operands that come from HBM (the rings below hold 2-4 slices, less than one DRAM round trip under load)
 __device__ __forceinline__ void tma_prefetch_2d(const void *tmap, int c0, int c1) {
@@ -165,6 +183,8 @@ struct TcGeom {
     long long m_total;
     int pf;        // flat (2-D map) operands: L2 prefetch distance in K-slices (0 = off)
     int xf_trunc;  // XF transform: truncating hi/lo split (split4_relu_trunc) instead of the round-to-nearest one
+    int epi_tma;   // TcPlan::epi_tma
+    int eslot, neslots;  // epilogue staging ring: bytes per slot (one 32-channel chunk of every epilogue tensor), slots
 };
 
 constexpr int SMEM_LIMIT = 232448;       // opt-in dynamic shared memory per CTA on sm_90 (227 KB)
@@ -178,36 +198,47 @@ constexpr uint32_t RAW_TILE_BYTES = 128 * 64 * 4;
 template <int BLOCK_N, bool ONE> __host__ __device__ constexpr int tc_stage_bytes() {
     return (ONE ? 1 : 2) * (A_TILE_BYTES + BLOCK_N * 128);
 }
-template <int BLOCK_N, bool XF, bool ONE> constexpr int tc_smem(int stages) {
-    return 1024 + stages * tc_stage_bytes<BLOCK_N, ONE>() + (XF ? 2 * (int)RAW_TILE_BYTES : 0) + 8 * (2 * stages + 4);
+// Epilogue staging (EPI_PLAIN, EPI_RES): a ring of slots, each one 32-channel chunk of the tile (128 rows) of every
+// epilogue tensor: [raw fp32 16 KB, 128B-swizzled | hi fp16 8 KB | lo fp16 8 KB, 64B-swizzled].  The raw part exists when
+// the layer has a residual or a raw output; the residual lands there and the raw output leaves from there.
+constexpr int EPI_RAW_BYTES = 128 * 32 * 4, EPI_HALF_BYTES = 128 * 32 * 2;
+constexpr int EPI_MAX_SLOTS = 24;
+constexpr int BAR_BYTES = 8 * (2 * 16 + 4 + 2 * EPI_MAX_SLOTS);   // up to 16 operand stages
+template <int BLOCK_N, bool XF, bool ONE> constexpr int tc_smem(int stages, int ring) {
+    return 1024 + stages * tc_stage_bytes<BLOCK_N, ONE>() + (XF ? 2 * (int)RAW_TILE_BYTES : 0) + ring + BAR_BYTES;
 }
-// STAGES: as many operand slots as fit 227 KB beside the XF staging ring
-template <int BLOCK_N, bool XF, bool ONE> constexpr int tc_stages() {
+// EPI_RES (the memory-bound conv3 layers): two operand stages, the rest is staging ring, so that a whole tile's residual
+// can be in flight during the tile's MMA.  EPI_PLAIN: a 32 KB ring beside as many stages as fit.  EPI_UP2 stores from
+// registers and has no ring.
+template <int BLOCK_N, int MODE, bool XF, bool ONE> constexpr int tc_ring() {
+    return MODE == EPI_UP2 ? 0 : MODE == EPI_RES ? (SMEM_LIMIT - tc_smem<BLOCK_N, XF, ONE>(2, 0)) / EPI_RAW_BYTES * EPI_RAW_BYTES
+                                                 : 2 * EPI_RAW_BYTES;
+}
+template <int BLOCK_N, int MODE, bool XF, bool ONE> constexpr int tc_stages() {
+    if (MODE == EPI_RES) return 2;
     int s = 1;
-    while (tc_smem<BLOCK_N, XF, ONE>(s + 1) <= SMEM_LIMIT) ++s;
+    while (tc_smem<BLOCK_N, XF, ONE>(s + 1, tc_ring<BLOCK_N, MODE, XF, ONE>()) <= SMEM_LIMIT) ++s;
     return s;
 }
-static_assert(tc_stages<128, false, false>() == 3 && tc_stages<128, true, false>() == 2 && tc_stages<64, false, false>() == 4 &&
-                  tc_stages<64, true, false>() == 3 && tc_stages<32, false, false>() == 5,
+static_assert(tc_stages<128, EPI_PLAIN, false, false>() == 3 && tc_stages<128, EPI_PLAIN, true, false>() == 2 &&
+                  tc_stages<64, EPI_PLAIN, false, false>() == 4 && tc_stages<64, EPI_PLAIN, true, false>() == 2 &&
+                  tc_stages<32, EPI_PLAIN, false, false>() == 4 && tc_stages<128, EPI_UP2, false, false>() == 3,
               "two-plane stage counts");
+static_assert(tc_ring<128, EPI_RES, false, false>() == 6 * EPI_RAW_BYTES, "EPI_RES ring: a 64 KB residual tile in flight");
+static_assert(tc_stages<32, EPI_PLAIN, false, true>() <= 16 && tc_ring<32, EPI_RES, false, true>() / EPI_RAW_BYTES <= EPI_MAX_SLOTS,
+              "barrier area");
 
-// Output element offsets of one accumulator row (pixel); -1 = no such pixel.
+// Output element offsets of one accumulator row (pixel) for EPI_UP2; -1 = no such pixel.
 struct PixOff {
-    long long res = -1, raw = -1, spl = -1, skip = -1;
+    long long raw = -1, spl = -1, skip = -1;
 };
 
-template <int MODE>
-__device__ __forceinline__ PixOff pix_offsets(const ConvParams &P, bool valid, int n, int oy, int ox) {
+__device__ __forceinline__ PixOff pix_offsets_up2(const ConvParams &P, bool valid, int n, int oy, int ox) {
     PixOff o;
     if (!valid) return o;
-    if (MODE == EPI_RES) o.res = n * P.res.sN + (long long)oy * P.res.sH + (long long)ox * P.res.sW;
     if (P.out_raw.p) o.raw = n * P.out_raw.sN + (long long)oy * P.out_raw.sH + (long long)ox * P.out_raw.sW;
-    if (MODE == EPI_UP2) {
-        o.spl = n * P.out_split.sN + (long long)(2 * oy) * P.out_split.sH + (long long)(2 * ox) * P.out_split.sW;
-        o.skip = n * P.skip.sN + (long long)(2 * oy) * P.skip.sH + (long long)(2 * ox) * P.skip.sW;
-    } else if (P.out_split.hi) {
-        o.spl = n * P.out_split.sN + (long long)oy * P.out_split.sH + (long long)ox * P.out_split.sW;
-    }
+    o.spl = n * P.out_split.sN + (long long)(2 * oy) * P.out_split.sH + (long long)(2 * ox) * P.out_split.sW;
+    o.skip = n * P.skip.sN + (long long)(2 * oy) * P.skip.sH + (long long)(2 * ox) * P.skip.sW;
     return o;
 }
 
@@ -231,32 +262,30 @@ __device__ __forceinline__ __half2 bits_h2(float f) {
     return *reinterpret_cast<const __half2 *>(&u);
 }
 
-// Channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  The global reads were issued earlier into
-// `pre`: EPI_RES the residual pair {r.x, r.y}; EPI_UP2 the skip pairs of the four output pixels, hi (and, unless ONE,
-// lo) as fp16x2 bits, [d * planes + plane].
-template <int MODE, bool ONE>
-__device__ __forceinline__ void epi_finish2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, float2 s, float2 b,
-                                            const float *pre) {
-    if constexpr (MODE == EPI_RES) { v0 += pre[0]; v1 += pre[1]; }
+// EPI_UP2, channels c, c+1 of one pixel: v already carries the weight exponent's 2^-e.  The skip pairs of the four
+// output pixels were read earlier into `pre`: hi (and, unless ONE, lo) as fp16x2 bits, [d * planes + plane].
+template <bool ONE>
+__device__ __forceinline__ void epi_finish2_up2(const ConvParams &P, const PixOff &o, int c, float v0, float v1, const float *pre) {
     if (o.raw >= 0) *reinterpret_cast<float2 *>(P.out_raw.p + o.raw + c) = make_float2(v0, v1);
-    if constexpr (MODE == EPI_UP2) {
 #pragma unroll
-        for (int d = 0; d < 4; ++d) {
-            const long long oo = o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c;
-            if constexpr (ONE) {
-                const __half2 sh = bits_h2(pre[d]);
-                store_split2<true>(P.out_split, oo, v0 + __half2float(sh.x), v1 + __half2float(sh.y));
-            } else {
-                const __half2 sh = bits_h2(pre[2 * d]), sl = bits_h2(pre[2 * d + 1]);
-                store_split2<false>(P.out_split, oo, v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
-            }
+    for (int d = 0; d < 4; ++d) {
+        const long long oo = o.spl + (d >> 1) * P.out_split.sH + (d & 1) * P.out_split.sW + c;
+        if constexpr (ONE) {
+            const __half2 sh = bits_h2(pre[d]);
+            store_split2<true>(P.out_split, oo, v0 + __half2float(sh.x), v1 + __half2float(sh.y));
+        } else {
+            const __half2 sh = bits_h2(pre[2 * d]), sl = bits_h2(pre[2 * d + 1]);
+            store_split2<false>(P.out_split, oo, v0 + join_f16(sh.x, sl.x), v1 + join_f16(sh.y, sl.y));
         }
-    } else if (o.spl >= 0) {
-        float t0 = v0, t1 = v1;
-        if (P.scale) { t0 = t0 * s.x + b.x; t1 = t1 * s.y + b.y; }
-        if (P.relu) { t0 = fmaxf(t0, 0.f); t1 = fmaxf(t1, 0.f); }
-        store_split2<ONE>(P.out_split, o.spl + c, t0, t1);
     }
+}
+
+// Byte offsets inside a staging slot of the fragment pair (row, channels 8 jj + 2 q, +1) of a 32-channel chunk
+__device__ __forceinline__ int stg_raw_off(int row, int jj, int q) {   // fp32 [128][32], 128B swizzle
+    return row * 128 + (((2 * jj + (q >> 1)) ^ (row & 7)) << 4) + (q & 1) * 8;
+}
+__device__ __forceinline__ int stg_half_off(int row, int jj, int q) {  // fp16 [128][32], 64B swizzle
+    return row * 64 + ((jj ^ ((row >> 1) & 3)) << 4) + q * 4;
 }
 
 template <int BLOCK_N, int STAGES, int MODE, bool XF, bool ONE>
@@ -264,18 +293,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
           const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
           const __grid_constant__ CUtensorMap tm_a2_hi, const __grid_constant__ CUtensorMap tm_a2_lo,
+          const __grid_constant__ CUtensorMap tm_res, const __grid_constant__ CUtensorMap tm_o_raw,
+          const __grid_constant__ CUtensorMap tm_o_hi, const __grid_constant__ CUtensorMap tm_o_lo,
           const ConvParams P, const TcGeom G) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int STAGE_BYTES = tc_stage_bytes<BLOCK_N, ONE>();
     constexpr int PLANES = ONE ? 1 : 2;
+    constexpr int RING = tc_ring<BLOCK_N, MODE, XF, ONE>();
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t raw_base = smem_base + STAGES * STAGE_BYTES;             // XF: 2-slot ring of raw fp32 [128][64] tiles
-    const uint32_t bar_base = raw_base + (XF ? 2 * RAW_TILE_BYTES : 0u);
-    // barriers: full[STAGES], empty[STAGES], raw_full[2], raw_empty[2]
+    const uint32_t ring_base = raw_base + (XF ? 2 * RAW_TILE_BYTES : 0u);  // epilogue staging ring
+    const uint32_t bar_base = ring_base + RING;
+    // barriers: full[STAGES], empty[STAGES], raw_full[2], raw_empty[2], epi_full[neslots], epi_free[neslots]
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
     auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + r); };
     auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * STAGES + 2 + r); };
+    auto efull_bar = [&](int e) { return bar_base + 8u * (2 * STAGES + 4 + e); };
+    auto efree_bar = [&](int e) { return bar_base + 8u * (2 * STAGES + 4 + EPI_MAX_SLOTS + e); };
+    const bool has_raw = MODE == EPI_RES || P.out_raw.p;   // the slot has a raw part
 
     // warp index broadcast from lane 0: provably warp-uniform, so the role branches below do not count as divergent
     // paths around the wgmma (ptxas would otherwise serialise them)
@@ -283,6 +319,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), XF ? 1 + XF_WARPS : 1); mbar_init(empty_bar(s), CONS_WARPS); }
         if (XF) for (int r = 0; r < 2; ++r) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), XF_WARPS); }
+        if (RING) for (int e = 0; e < G.neslots; ++e) { mbar_init(efull_bar(e), 1); mbar_init(efree_bar(e), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -295,7 +332,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
     if (warp == 0) {
         // ===================== TMA producer =====================
         if (lane == 0) {
-            int it_global = 0;
+            int it_global = 0, ec = 0;
             // L2 prefetch cursor, G.pf K-slices ahead of the loads through the same (tile, slice) sequence.  Flat layers
             // only: their A operand is a whole encoder tensor streamed from HBM.
             const bool pf_on = G.flat && G.pf > 0;
@@ -372,6 +409,25 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                     }
                     tma_3d(b_hi, &tm_w_hi, full_bar(s), kc * 64, tn * BLOCK_N, tap);
                     if constexpr (!ONE) tma_3d(b_lo, &tm_w_lo, full_bar(s), kc * 64, tn * BLOCK_N, tap);
+                    if constexpr (MODE == EPI_RES) {
+                        // the tile's residual, one 32-channel chunk per staging slot, behind the tile's last K-slice
+                        // (a slot may free up only once this tile's first chunks are stored, so every operand of the
+                        // tile must be on its way first): in flight while the tile's MMA runs.  res may alias out_raw
+                        // element for element: each (tile, chunk) is loaded here before the same CTA stores it from the
+                        // same slot, and no two tiles share an address, so a load never sees another tile's store.
+                        if (it == kiters - 1 && G.epi_tma) {
+                            const uint32_t bytes = (uint32_t)((G.flat ? 128 : G.bw * G.bh) * 128);
+                            for (int q = 0; q < BLOCK_N / 32; ++q, ++ec) {
+                                const int e = ec % G.neslots;
+                                mbar_wait(efree_bar(e), ((uint32_t)(ec / G.neslots) & 1u) ^ 1u);
+                                mbar_expect_tx(efull_bar(e), bytes);
+                                const uint32_t dst = ring_base + e * G.eslot;
+                                const int c = tn * BLOCK_N + 32 * q;
+                                if (G.flat) tma_2d(dst, &tm_res, efull_bar(e), c, (int)m0);
+                                else tma_4d(dst, &tm_res, efull_bar(e), c, x0, y0, n_img);
+                            }
+                        }
+                    }
                 }
             }
         }
@@ -477,7 +533,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
             __syncwarp();
             if (lane == 0) mbar_arrive(empty_bar(s));
         };
-        int it_global = 0;
+        int it_global = 0, ec = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int tm = tile / G.tiles_n, tn = tile - tm * G.tiles_n;
 #pragma unroll
@@ -516,62 +572,47 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                 for (int j = 0; j < NR; ++j) sum[j] += acc[j];
             }
             // ---- epilogue straight from the fragment: rows ra, ra + 8; two consecutive channels per register pair.
-            // acc is dead until the next tile's first wgmma (scale-d = 0), so it holds what the epilogue reads from global
-            // memory: all of a batch's reads are issued before its first store.  The compiler cannot hoist them itself,
-            // since res may alias out_raw and skip may alias out_split.
+            auto flat_pix = [&](int row, int &n_img, int &oy, int &ox) {
+                const long long m = (long long)tm * 128 + row;
+                if (m >= G.m_total) return false;
+                const long long hw = (long long)P.ho * P.wo;
+                n_img = (int)(m / hw);
+                const int r = (int)(m - (long long)n_img * hw);
+                oy = r / P.wo; ox = r - oy * P.wo;
+                return true;
+            };
+            const int per_img = G.tiles_x * G.tiles_y;
+            const int n_box = G.flat ? 0 : tm / per_img, r_box = tm - n_box * per_img;
+            const int y_box = G.flat ? 0 : (r_box / G.tiles_x) * G.bh, x_box = G.flat ? 0 : (r_box - (r_box / G.tiles_x) * G.tiles_x) * G.bw;
+            bool vrow[2];
             PixOff po[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = ra + 8 * h;
-                bool valid;
-                int n_img, oy, ox;
-                if (G.flat) {
-                    const long long m = (long long)tm * 128 + row;
-                    valid = m < G.m_total;
-                    const long long hw = (long long)P.ho * P.wo;
-                    n_img = valid ? (int)(m / hw) : 0;
-                    const int r = valid ? (int)(m - (long long)n_img * hw) : 0;
-                    oy = r / P.wo; ox = r - oy * P.wo;
-                } else {
-                    const int per_img = G.tiles_x * G.tiles_y;
-                    n_img = tm / per_img;
-                    const int r = tm - n_img * per_img;
-                    const int ty = r / G.tiles_x, tx = r - ty * G.tiles_x;
+                int n_img = n_box, oy = 0, ox = 0;
+                if (G.flat) vrow[h] = flat_pix(row, n_img, oy, ox);
+                else {
                     const int py = row / G.bw, px = row - py * G.bw;
-                    oy = ty * G.bh + py; ox = tx * G.bw + px;
-                    valid = row < G.bw * G.bh && oy < P.ho && ox < P.wo;
+                    oy = y_box + py; ox = x_box + px;
+                    vrow[h] = row < G.bw * G.bh && oy < P.ho && ox < P.wo;
                 }
-                po[h] = pix_offsets<MODE>(P, valid, n_img, oy, ox);
+                if constexpr (MODE == EPI_UP2) po[h] = pix_offsets_up2(P, vrow[h], n_img, oy, ox);
             }
-            const bool bn = MODE != EPI_UP2 && P.scale && P.out_split.hi;
-            // EPI_RES: the whole fragment's residual, one float2 per register pair (one round trip per tile)
-            if constexpr (MODE == EPI_RES) {
+            if constexpr (MODE == EPI_UP2) {
+                // acc is dead until the next tile's first wgmma (scale-d = 0), so it holds the skip pairs the epilogue
+                // reads: batches of JB column groups j, 2 rows x 4 output pixels x planes per j, all of a batch's reads
+                // issued before its first store (four round trips per tile).  The compiler cannot hoist them itself,
+                // since skip may alias out_split.  JB is the largest batch that stays within 168 registers without
+                // spilling at BLOCK_N = 128.
+                constexpr int JB = NR / 16;
+                static_assert((BLOCK_N / 8) % JB == 0, "epilogue batch must divide the column groups");
 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; ++j) {
-                    const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
+                for (int j0 = 0; j0 < BLOCK_N / 8; j0 += JB) {
+                    float2 ws[JB];
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        if (po[h].res >= 0) {
-                            const float2 r = *reinterpret_cast<const float2 *>(P.res.p + po[h].res + c);
-                            acc[4 * j + 2 * h] = r.x; acc[4 * j + 2 * h + 1] = r.y;
-                        }
-                }
-            }
-            // Batches of JB column groups j, their per-channel scales loaded up front.  EPI_UP2: the skip pairs of a batch
-            // (2 rows x 4 output pixels x planes per j) go into acc, four round trips per tile.  The batch sizes are the
-            // largest that stay within 168 registers without spilling at BLOCK_N = 128.
-            constexpr int JB = MODE == EPI_UP2 ? NR / 16 : 2;
-            static_assert((BLOCK_N / 8) % JB == 0, "epilogue batch must divide the column groups");
-#pragma unroll
-            for (int j0 = 0; j0 < BLOCK_N / 8; j0 += JB) {
-                float2 ws[JB], sc[JB], sh[JB];
-#pragma unroll
-                for (int jj = 0; jj < JB; ++jj) {
-                    const int c = tn * BLOCK_N + 8 * (j0 + jj) + 2 * (lane & 3);
-                    ws[jj] = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
-                    sc[jj] = make_float2(1.f, 1.f); sh[jj] = make_float2(0.f, 0.f);
-                    if (bn) { sc[jj] = __ldg(reinterpret_cast<const float2 *>(P.scale + c)); sh[jj] = __ldg(reinterpret_cast<const float2 *>(P.shift + c)); }
-                    if constexpr (MODE == EPI_UP2) {
+                    for (int jj = 0; jj < JB; ++jj) {
+                        const int c = tn * BLOCK_N + 8 * (j0 + jj) + 2 * (lane & 3);
+                        ws[jj] = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
 #pragma unroll
                         for (int h = 0; h < 2; ++h)
                             if (po[h].skip >= 0)
@@ -583,20 +624,142 @@ k_conv_tc(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ C
                                     if constexpr (!ONE) pre[1] = ld_bits(P.skip.lo + so);
                                 }
                     }
+#pragma unroll
+                    for (int jj = 0; jj < JB; ++jj) {
+                        const int j = j0 + jj;
+                        const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            if (po[h].spl >= 0)
+                                epi_finish2_up2<ONE>(P, po[h], c, sum[4 * j + 2 * h] * ws[jj].x, sum[4 * j + 2 * h + 1] * ws[jj].y,
+                                                     &acc[(jj * 2 + h) * 4 * PLANES]);
+                    }
                 }
+            } else {
+                // Chunks of 32 channels through the staging ring: the fragment goes into the slot (added to the residual
+                // TMA put there), then one thread hands the slot to TMA as bulk tensor stores, which clip rows past
+                // m_total and pixels past ho / wo.  Per element: sum * oscale (+ res) -> raw ; BN, ReLU -> split.
+                const bool bn = P.scale && P.out_split.hi;
+                const int q4 = lane & 3, ct = threadIdx.x - 128;
 #pragma unroll
-                for (int jj = 0; jj < JB; ++jj) {
-                    const int j = j0 + jj;
-                    const int c = tn * BLOCK_N + 8 * j + 2 * (lane & 3);
+                for (int q = 0; q < BLOCK_N / 32; ++q, ++ec) {
+                    const int e = ec % G.neslots;
+                    const uint32_t eph = (uint32_t)(ec / G.neslots) & 1u;
+                    const uint32_t s_raw = ring_base + e * G.eslot, s_hi = s_raw + (has_raw ? EPI_RAW_BYTES : 0),
+                                   s_lo = s_hi + EPI_HALF_BYTES;
+                    uint8_t *g_raw = smem_raw + (s_raw - smem_u32(smem_raw)), *g_hi = smem_raw + (s_hi - smem_u32(smem_raw)),
+                            *g_lo = g_hi + EPI_HALF_BYTES;
+                    const int cq = tn * BLOCK_N + 32 * q;
+                    if (G.epi_tma) {
+                        if (MODE == EPI_RES) mbar_wait(efull_bar(e), eph);   // the chunk's residual has landed
+                        else mbar_wait(efree_bar(e), eph ^ 1u);             // the slot's previous store has read it
+                    } else if (MODE == EPI_RES) {                           // cropped view: copy the residual in
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        if (po[h].raw >= 0 || po[h].spl >= 0)
-                            epi_finish2<MODE, ONE>(P, po[h], c, sum[4 * j + 2 * h] * ws[jj].x, sum[4 * j + 2 * h + 1] * ws[jj].y,
-                                                   sc[jj], sh[jj],
-                                                   MODE == EPI_UP2 ? &acc[(jj * 2 + h) * 4 * PLANES] : &acc[4 * j + 2 * h]);
+                        for (int i = 0; i < 4; ++i) {
+                            const int p = ct + 256 * i, row = p >> 3, k = p & 7;
+                            int n_img, oy, ox;
+                            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                            if (flat_pix(row, n_img, oy, ox))
+                                v = *reinterpret_cast<const float4 *>(P.res.p + n_img * P.res.sN + (long long)oy * P.res.sH +
+                                                                      (long long)ox * P.res.sW + cq + 4 * k);
+                            *reinterpret_cast<float4 *>(g_raw + row * 128 + ((k ^ (row & 7)) << 4)) = v;
+                        }
+                        consumers_sync();
+                    }
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int j = 4 * q + jj;
+                        const int c = cq + 8 * jj + 2 * q4;
+                        const float2 ws = __ldg(reinterpret_cast<const float2 *>(P.w.oscale + c));
+                        float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
+                        if (bn) { sc = __ldg(reinterpret_cast<const float2 *>(P.scale + c)); sh = __ldg(reinterpret_cast<const float2 *>(P.shift + c)); }
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int row = ra + 8 * h;
+                            float v0 = sum[4 * j + 2 * h] * ws.x, v1 = sum[4 * j + 2 * h + 1] * ws.y;
+                            const int ro = stg_raw_off(row, jj, q4);
+                            if constexpr (MODE == EPI_RES) {
+                                const float2 r = *reinterpret_cast<const float2 *>(g_raw + ro);
+                                v0 += r.x; v1 += r.y;
+                            }
+                            if (P.out_raw.p) *reinterpret_cast<float2 *>(g_raw + ro) = make_float2(v0, v1);
+                            if (P.out_split.hi) {
+                                float t0 = v0, t1 = v1;
+                                if (P.scale) { t0 = t0 * sc.x + sh.x; t1 = t1 * sc.y + sh.y; }
+                                if (P.relu) { t0 = fmaxf(t0, 0.f); t1 = fmaxf(t1, 0.f); }
+                                unsigned int *flag = vrow[h] ? P.out_split.flag : nullptr;   // rows that are stored
+                                const int so = stg_half_off(row, jj, q4);
+                                if constexpr (ONE) {
+                                    *reinterpret_cast<__half2 *>(g_hi + so) = __halves2half2(hi_f32(t0, flag), hi_f32(t1, flag));
+                                } else {
+                                    __half h0, l0, h1, l1;
+                                    split_f32(t0, h0, l0, flag);
+                                    split_f32(t1, h1, l1, flag);
+                                    *reinterpret_cast<__half2 *>(g_hi + so) = __halves2half2(h0, h1);
+                                    *reinterpret_cast<__half2 *>(g_lo + so) = __halves2half2(l0, l1);
+                                }
+                            }
+                        }
+                    }
+                    if (G.epi_tma) {
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> visible to TMA
+                        consumers_sync();
+                        if (threadIdx.x == 128) {
+                            if (G.flat) {
+                                if (P.out_raw.p) tma_store_2d(&tm_o_raw, s_raw, cq, tm * 128);
+                                if (P.out_split.hi) {
+                                    tma_store_2d(&tm_o_hi, s_hi, cq, tm * 128);
+                                    if constexpr (!ONE) tma_store_2d(&tm_o_lo, s_lo, cq, tm * 128);
+                                }
+                            } else {
+                                if (P.out_raw.p) tma_store_4d(&tm_o_raw, s_raw, cq, x_box, y_box, n_box);
+                                if (P.out_split.hi) {
+                                    tma_store_4d(&tm_o_hi, s_hi, cq, x_box, y_box, n_box);
+                                    if constexpr (!ONE) tma_store_4d(&tm_o_lo, s_lo, cq, x_box, y_box, n_box);
+                                }
+                            }
+                            bulk_commit();
+                            // a slot goes back (to the producer's residual load, or to the next chunk written into it)
+                            // once its store has read it: the previous chunk's, so that this store stays in flight
+                            if (G.neslots > 1) {
+                                bulk_wait_read<1>();
+                                if (ec > 0) mbar_arrive(efree_bar((ec - 1) % G.neslots));
+                            } else {
+                                bulk_wait_read<0>();
+                                mbar_arrive(efree_bar(e));
+                            }
+                        }
+                    } else {  // cropped view: copy the chunk out, 16 bytes per thread and step
+                        consumers_sync();
+                        if (P.out_raw.p)
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const int p = ct + 256 * i, row = p >> 3, k = p & 7;
+                                int n_img, oy, ox;
+                                if (flat_pix(row, n_img, oy, ox))
+                                    *reinterpret_cast<float4 *>(P.out_raw.p + n_img * P.out_raw.sN + (long long)oy * P.out_raw.sH +
+                                                                (long long)ox * P.out_raw.sW + cq + 4 * k) =
+                                        *reinterpret_cast<const float4 *>(g_raw + row * 128 + ((k ^ (row & 7)) << 4));
+                            }
+                        if (P.out_split.hi)
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                const int p = ct + 256 * i, row = p >> 2, k = p & 3;
+                                int n_img, oy, ox;
+                                if (flat_pix(row, n_img, oy, ox)) {
+                                    const long long o = n_img * P.out_split.sN + (long long)oy * P.out_split.sH +
+                                                        (long long)ox * P.out_split.sW + cq + 8 * k;
+                                    const int so = row * 64 + ((k ^ ((row >> 1) & 3)) << 4);
+                                    *reinterpret_cast<uint4 *>(P.out_split.hi + o) = *reinterpret_cast<const uint4 *>(g_hi + so);
+                                    if constexpr (!ONE) *reinterpret_cast<uint4 *>(P.out_split.lo + o) = *reinterpret_cast<const uint4 *>(g_lo + so);
+                                }
+                            }
+                        consumers_sync();
+                    }
                 }
             }
         }
+        if (threadIdx.x == 128) bulk_wait<0>();   // every bulk store complete before the CTA exits
     }
 }
 
@@ -808,18 +971,38 @@ static EncodeTiledFn encode_fn() {
     return fn;
 }
 
-static bool encode(unsigned char *dst, void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides_bytes,
-                   const cuuint32_t *box, const cuuint32_t *estr, bool raw_f32 = false) {
+static bool encode(unsigned char *dst, const void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides_bytes,
+                   const cuuint32_t *box, const cuuint32_t *estr, CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                   CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return false;
     alignas(64) CUtensorMap tm;
-    CUresult r = fn(&tm, raw_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, base,
-                    dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    raw_f32 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = fn(&tm, dt, (cuuint32_t)rank, const_cast<void *>(base), dims, strides_bytes, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return false;
     memcpy(dst, &tm, sizeof(tm));
     return true;
+}
+constexpr CUtensorMapDataType TM_F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+
+// One epilogue tensor (element size es, strides in elements) as 32-channel boxes of an M-tile: flat tiles a 2-D
+// [pixels, channels] map over the view's rows, box tiles a 4-D (C, bw, bh, 1) box.  fp32 boxes (128 B per pixel) are
+// 128B-swizzled, fp16 boxes (64 B per pixel) 64B-swizzled, the layouts stg_raw_off / stg_half_off write.
+static bool encode_epi(unsigned char *dst, const void *base, long long sN, int sH, int sW, int es, const ConvParams &P,
+                       const TcPlan &plan) {
+    const CUtensorMapDataType dt = es == 4 ? TM_F32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const CUtensorMapSwizzle sw = es == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    cuuint32_t ones[4] = {1, 1, 1, 1};
+    if (plan.flat) {
+        cuuint64_t dims[2] = {(cuuint64_t)P.w.cout, (cuuint64_t)((long long)P.B * P.ho * P.wo)};
+        cuuint64_t str[1] = {(cuuint64_t)sW * es};
+        cuuint32_t box[2] = {32, 128};
+        return encode(dst, base, 2, dims, str, box, ones, dt, sw);
+    }
+    cuuint64_t dims[4] = {(cuuint64_t)P.w.cout, (cuuint64_t)P.wo, (cuuint64_t)P.ho, (cuuint64_t)P.B};
+    cuuint64_t str[3] = {(cuuint64_t)sW * es, (cuuint64_t)sH * es, (cuuint64_t)sN * es};
+    cuuint32_t box[4] = {32, (cuuint32_t)plan.bw, (cuuint32_t)plan.bh, 1};
+    return encode(dst, base, 4, dims, str, box, ones, dt, sw);
 }
 
 static int g_force_block_n = 0;
@@ -895,7 +1078,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         } else {
             cuuint64_t rdims[2] = {(cuuint64_t)P.a_raw.c, (cuuint64_t)((long long)P.B * P.a_raw.h * P.a_raw.w)};
             cuuint64_t rstr[1] = {(cuuint64_t)P.a_raw.sW * 4};
-            if (!encode(plan.tmap_a_hi, P.a_raw.p, 2, rdims, rstr, box, ones, true)) return false;
+            if (!encode(plan.tmap_a_hi, P.a_raw.p, 2, rdims, rstr, box, ones, TM_F32, CU_TENSOR_MAP_SWIZZLE_NONE)) return false;
         }
         plan.bw = 128; plan.bh = 1; plan.tiles_x = plan.tiles_y = 0;
         if (two) {
@@ -929,7 +1112,7 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         } else {
             cuuint64_t rdims[4] = {(cuuint64_t)P.a_raw.c, (cuuint64_t)P.a_raw.w, (cuuint64_t)P.a_raw.h, (cuuint64_t)P.B};
             cuuint64_t rstr[3] = {(cuuint64_t)P.a_raw.sW * 4, (cuuint64_t)P.a_raw.sH * 4, (cuuint64_t)P.a_raw.sN * 4};
-            if (!encode(plan.tmap_a_hi, P.a_raw.p, 4, rdims, rstr, box, estr, true)) return false;
+            if (!encode(plan.tmap_a_hi, P.a_raw.p, 4, rdims, rstr, box, estr, TM_F32, CU_TENSOR_MAP_SWIZZLE_NONE)) return false;
         }
         if (two) {
             const int s2 = P.a2_stride;
@@ -949,26 +1132,56 @@ bool tc_plan(const ConvParams &P, TcPlan &plan) {
         if (!encode(plan.tmap_w_hi, w.hi, 3, dims, str, box, ones)) return false;
         if (!one && !encode(plan.tmap_w_lo, w.lo, 3, dims, str, box, ones)) return false;
     }
+    if (!P.up2) {
+        // epilogue tensors: 16-byte aligned bases and strides (TMA, and the staged copy of a cropped flat view)
+        auto al16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+        if (P.res.p && (!al16(P.res.p) || P.res.sW % 4 || P.res.sH % 4 || P.res.sN % 4)) return false;
+        if (P.out_raw.p && (!al16(P.out_raw.p) || P.out_raw.sW % 4 || P.out_raw.sH % 4 || P.out_raw.sN % 4)) return false;
+        if (P.out_split.hi && (!al16(P.out_split.hi) || (!one && !al16(P.out_split.lo)) || P.out_split.sW % 8 ||
+                               P.out_split.sH % 8 || P.out_split.sN % 8)) return false;
+        // a flat tile is 128 consecutive pixels: one TMA box only where the view's rows are dense
+        auto rows_dense = [&](long long sN, int sH, int sW) { return (long long)sW * P.wo == sH && (long long)sH * P.ho == sN; };
+        plan.epi_tma = 1;
+        if (plan.flat && ((P.res.p && !rows_dense(P.res.sN, P.res.sH, P.res.sW)) ||
+                          (P.out_raw.p && !rows_dense(P.out_raw.sN, P.out_raw.sH, P.out_raw.sW)) ||
+                          (P.out_split.hi && !rows_dense(P.out_split.sN, P.out_split.sH, P.out_split.sW))))
+            plan.epi_tma = 0;
+        if (plan.epi_tma) {
+            if (P.res.p && !encode_epi(plan.tmap_res, P.res.p, P.res.sN, P.res.sH, P.res.sW, 4, P, plan)) return false;
+            if (P.out_raw.p && !encode_epi(plan.tmap_out_raw, P.out_raw.p, P.out_raw.sN, P.out_raw.sH, P.out_raw.sW, 4, P, plan))
+                return false;
+            if (P.out_split.hi) {
+                const SplitRef &o = P.out_split;
+                if (!encode_epi(plan.tmap_out_hi, o.hi, o.sN, o.sH, o.sW, 2, P, plan)) return false;
+                if (!one && !encode_epi(plan.tmap_out_lo, o.lo, o.sN, o.sH, o.sW, 2, P, plan)) return false;
+            }
+        }
+    }
     plan.ok = true;
     return true;
 }
 
 template <int BLOCK_N, int MODE, bool XF, bool ONE>
-static void launch_tm(const ConvParams &P, const TcPlan &plan, const TcGeom &G, cudaStream_t s) {
-    constexpr int STAGES = tc_stages<BLOCK_N, XF, ONE>();
-    constexpr int smem = tc_smem<BLOCK_N, XF, ONE>(STAGES);
+static void launch_tm(const ConvParams &P, const TcPlan &plan, TcGeom G, cudaStream_t s) {
+    constexpr int STAGES = tc_stages<BLOCK_N, MODE, XF, ONE>();
+    constexpr int RING = tc_ring<BLOCK_N, MODE, XF, ONE>();
+    constexpr int smem = tc_smem<BLOCK_N, XF, ONE>(STAGES, RING);
     static_assert(smem <= SMEM_LIMIT, "shared memory budget exceeded");
     static bool attr = false;
     if (!attr) {
         HVN_CUDA(cudaFuncSetAttribute(k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr = true;
     }
+    G.eslot = (MODE == EPI_RES || P.out_raw.p ? EPI_RAW_BYTES : 0) + (P.out_split.hi ? (ONE ? 1 : 2) * EPI_HALF_BYTES : 0);
+    G.neslots = RING && G.eslot ? std::min(RING / G.eslot, EPI_MAX_SLOTS) : 1;
+    if (RING && G.eslot) HVN_CHECK(G.neslots >= 1, -1, "conv_tc: epilogue staging ring too small");
     const int grid = std::min(G.tiles_m * G.tiles_n, num_sms());
-    CUtensorMap a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo;
-    memcpy(&a_hi, plan.tmap_a_hi, 128); memcpy(&a_lo, plan.tmap_a_lo, 128);
-    memcpy(&w_hi, plan.tmap_w_hi, 128); memcpy(&w_lo, plan.tmap_w_lo, 128);
-    memcpy(&a2_hi, plan.tmap_a2_hi, 128); memcpy(&a2_lo, plan.tmap_a2_lo, 128);
-    k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE><<<grid, TC_THREADS, smem, s>>>(a_hi, a_lo, w_hi, w_lo, a2_hi, a2_lo, P, G);
+    CUtensorMap t[10];
+    const unsigned char *src[10] = {plan.tmap_a_hi, plan.tmap_a_lo, plan.tmap_w_hi, plan.tmap_w_lo, plan.tmap_a2_hi,
+                                    plan.tmap_a2_lo, plan.tmap_res, plan.tmap_out_raw, plan.tmap_out_hi, plan.tmap_out_lo};
+    for (int i = 0; i < 10; ++i) memcpy(&t[i], src[i], 128);
+    k_conv_tc<BLOCK_N, STAGES, MODE, XF, ONE><<<grid, TC_THREADS, smem, s>>>(t[0], t[1], t[2], t[3], t[4], t[5], t[6], t[7], t[8],
+                                                                            t[9], P, G);
     g_last_dispatch = BLOCK_N | MODE << 8 | (XF ? 1 : 0) << 12 | (ONE ? 1 : 0) << 13;
 }
 
@@ -1038,6 +1251,7 @@ void tc_launch(const ConvParams &P, const TcPlan &plan, cudaStream_t s) {
     G.tiles_n = P.w.cout / plan.block_n;
     G.xf_trunc = g_xf_trunc;
     G.pf = g_pf;
+    G.epi_tma = plan.epi_tma;
     if (plan.single) {
         switch (plan.block_n) {
         case 128: launch_t<128, true>(P, plan, G, s); break;
